@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py -- frames/s of the Deformable-DETR R50 hot path (BASELINE.json metric) on N B200s.
+"""bench.py -- frames/s of the Deformable-DETR R50 hot path (BASELINE.json metric) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one training pass of the hot path over one synthetic batch per GPU:
-forward (ResNet-50 -> 4-level input projection -> 6+6 deformable transformer on the sm_100a
+forward (ResNet-50 -> 4-level input projection -> 6+6 deformable transformer on the sm_90a
 MSDeformAttn kernels -> heads) + SetCriterion (Hungarian matching, focal / L1 / GIoU over 6 layers) +
 backward + [N>1: NCCL gradient all-reduce through DDP] + grad-clip(0.1) + AdamW, exactly the six hot
 lines of the reference's engine.train_one_epoch (src/trackformer/engine.py:126-151).
@@ -25,6 +25,10 @@ Output: ONE JSON line on rank 0 (see the driver contract), with
   cpu_baseline  the reference's pure-PyTorch path (oracle/torch_ref.py driving the same host-side model on
             the host cores), rank 0, N=1 only, bounded sample
 `--impl reference` prints the CPU arm as the main line (rank 0 only; other ranks exit 0).
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed (rank 0): the loss it returned and
+the gradient it produced, as DIR/<name>.npy (see dump_outputs).  The last timed step starts from the seeded initial
+weights and optimizer state (TrainingState), so its inputs are the same in every run and two builds run with the same
+arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -56,7 +60,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 def msda_alg_bytes(kind, dims):
@@ -78,12 +82,12 @@ def make_targets(batch, device, seed):
 
 
 def tensor_peak(tf32: bool):
-    """Dense tensor-pipe denominator for the precision actually used: the driver-measured sustained bf16 cuBLAS rate
-    (the step is long, MEASURED_PEAKS.json) halved for TF32 (half the bf16 rate on this part); strict fp32 has no
+    """Dense tensor-pipe denominator for the precision actually used: the measured sustained bf16 cuBLAS rate
+    (MEASURED_PEAKS.json, when present) halved for TF32 (half the bf16 rate on H100); strict fp32 has no
     tensor-pipe roofline."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    bf16 = 1400.0
-    src = "fallback 1.4 PFLOP/s bf16 sustained (B200_PROFILING.md)"
+    bf16 = 989.0
+    src = "H100 SXM data sheet, 989 TFLOP/s dense bf16, not measured"
     if os.path.exists(p):
         try:
             bf16 = float(json.load(open(p))["bf16_tflops_sustained"])
@@ -108,6 +112,51 @@ def dense_flops_per_step(step_fn):
         return None
     finally:
         fl._TCGEN05 = own
+
+
+DUMP_SAMPLES = 1 << 20
+
+
+class TrainingState:
+    """Copy of the trainable state -- parameters and optimizer state -- taken before the first training step.
+
+    The gradient reductions of the backward (float atomics in the MSDeformAttn backward and the split-token weight
+    gradient) round differently from run to run, and AdamW, which divides every gradient by its own running magnitude,
+    plus the Hungarian matching turn those last-bit differences into different weights within a few steps.  restore()
+    puts the initial state back, so that a step run after it computes from the same weights in every run."""
+
+    def __init__(self, params, optimizer):
+        self.params, self.optimizer = list(params), optimizer
+        self.values = [p.detach().clone() for p in self.params]
+        self.opt_state = None
+        if optimizer is not None and hasattr(optimizer, "exp_avg"):          # flat AdamW: state exists from the start
+            self.opt_state = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in optimizer.state_dict().items()}
+
+    def restore(self):
+        with torch.no_grad():
+            torch._foreach_copy_([p.data for p in self.params], self.values)
+        if self.opt_state is not None:
+            self.optimizer.load_state_dict(self.opt_state)
+        elif self.optimizer is not None:
+            self.optimizer.state.clear()                                      # torch optimizers create it lazily
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes every tensor of `arrays` as out_dir/<name>.npy: scalars as float64, everything else as a flat float32
+    vector.  Vectors longer than DUMP_SAMPLES are reduced to the values at DUMP_SAMPLES fixed positions drawn from a
+    seeded generator (the same positions in every run), which keeps the dump at a few MB."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach()
+        if t.numel() == 1:
+            np.save(os.path.join(out_dir, name + ".npy"), t.reshape(()).double().cpu().numpy())
+            continue
+        flat = t.reshape(-1).float()
+        if flat.numel() > DUMP_SAMPLES:
+            idx = torch.randint(0, flat.numel(), (DUMP_SAMPLES,), generator=torch.Generator().manual_seed(0))
+            flat = flat[idx.sort().values.to(flat.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), flat.cpu().numpy())
 
 
 def golden_parity(dev):
@@ -311,6 +360,7 @@ def c5_arm(args, rank, local_rank, world):
             dist.barrier(device_ids=[local_rank])
         torch.cuda.synchronize(dev)
 
+    initial = TrainingState(params, opt)
     sampler = ClockSampler(local_rank) if rank == 0 else None
     if sampler:
         sampler.start()
@@ -334,8 +384,19 @@ def c5_arm(args, rank, local_rank, world):
     if sampler:
         sampler.mark_begin()
     l0 = msda.launch_count()
-    ms_total = timed(lambda: step(dev_frames))
+    last = {"i": 0}
+
+    def timed_step():
+        last["i"] += 1
+        if last["i"] == args.steps:
+            initial.restore()              # the last step computes from the seeded initial state (TrainingState)
+        last["loss"] = step(dev_frames)
+    ms_total = timed(timed_step)
     launches = msda.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {
+            "loss": last["loss"],
+            "grad_sample": torch.cat([p.grad.reshape(-1) for p in params if p.grad is not None])})
     if sampler:
         sampler.mark_end()
     clocks = sampler.stop() if sampler else None
@@ -398,6 +459,8 @@ def main():
                          "previous frame (eager: the track-query injection draws from the host RNG, like the reference)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-steps", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (see dump_outputs)")
     args = ap.parse_args()
     _claim_stdout()
 
@@ -429,7 +492,7 @@ def main():
         emit(line)
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     assert torch.cuda.is_available(), "bench.py needs a CUDA device (no CPU fallback for the product path)"
     if args.workload == "c5":
         return c5_arm(args, rank, local_rank, world)
@@ -449,7 +512,7 @@ def main():
     from trackformer_b200 import ext, msda_function
     from trackformer_b200.model_factory import build_model, default_args
     from trackformer_b200.train_step import TrainStep
-    msda = ext.load()          # raises if the sm_100a extension is missing
+    msda = ext.load()          # raises if the sm_90a extension is missing
 
     torch.manual_seed(0)       # same seed on every rank -> identical replicas
     model, criterion, _ = build_model(default_args(device=str(dev)))
@@ -470,6 +533,9 @@ def main():
         flat = {"groups": reference_param_groups(model)}
     step = TrainStep(model, criterion, opt_factory, max_norm=0.1, use_graphs=not args.no_graphs,
                      example_frames=dev_frames, example_targets=None if args.two_graphs else targets, flat_adamw=flat)
+
+    initial = TrainingState([step.flat_param] if step.flat_param is not None else step.params,
+                            step.flat_optimizer if step.flat_optimizer is not None else step.optimizer)
 
     def barrier():
         if world > 1:
@@ -511,9 +577,18 @@ def main():
     # (1) device-resident throughput
     if sampler:
         sampler.mark_begin()
-    ms_total = timed(lambda: step(dev_frames, targets), args.steps)
+    last = {"i": 0}
+
+    def timed_step():
+        last["i"] += 1
+        if last["i"] == args.steps:
+            initial.restore()              # the last step computes from the seeded initial state (TrainingState)
+        last["loss"] = step(dev_frames, targets)
+    ms_total = timed(timed_step, args.steps)
     if sampler:
         sampler.mark_end()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"loss": last["loss"], "grad_sample": step.flat_grad})
     clocks = sampler.stop() if sampler else None
     value = bpg * world * args.steps / (ms_total / 1e3)
 
@@ -603,7 +678,7 @@ def main():
                     "mean_launch_us": dom["mean_us"], "alg_bytes_per_launch": dom["alg_bytes"],
                     "note": "algorithmic (compulsory) bytes / CUDA-event launch time, every launch bracketed by events in an "
                             "eager replay of the timed step (graph replays cannot host per-kernel events); "
-                            "the gather itself is L1-wavefront bound, see DESIGN.md"}
+                            "the gather itself is L1-wavefront bound"}
     # second yardstick: the measured L1-data-stage ceiling for gather-shaped LDG.128 requests (tools/l1_gather_peak.py)
     l1_roofline = None
     l1_path = os.path.join(ROOT, "profiles", "l1_gather_peak.json")
@@ -660,8 +735,8 @@ def main():
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "tf32+f32" if tf32 else "f32", "data": "synthetic",
         "config": {"workload": workload, "global_batch": bpg * world, "parallelism": f"dp{world}",
-                   "dense_math": "TF32 tensor cores (cuDNN / cuBLAS / own tcgen05 Linear), fp32 accumulate" if tf32 else "strict fp32",
-                   "msda_math": "fp32 (hand-written sm_100a kernels)", "dropout": 0.1,
+                   "dense_math": "TF32 tensor cores (cuDNN / cuBLAS / own wgmma TF32 Linear), fp32 accumulate" if tf32 else "strict fp32",
+                   "msda_math": "fp32 (hand-written sm_90a kernels)", "dropout": 0.1,
                    "optimizer": "none" if args.no_optimizer else ("torch AdamW(fused)" if args.torch_adamw else "flat one-pass AdamW kernel, reference lr groups") + " + clip_grad_norm 0.1",
                    "execution": "eager" if args.no_graphs else
                    ("forward graph + loss (device Hungarian matching, no host sync) + backward graph" if args.two_graphs else
@@ -672,7 +747,7 @@ def main():
                                         "backward, fused residual+LayerNorm, column sums, ReLU+dropout, sampling prep, "
                                         "Hungarian matching, clip+AdamW), replayed from the graph except the optimizer",
                    "weights": "random init", "gt_boxes_per_frame": N_GT,
-                   "l2": "no explicit flush: one step streams >1 GB of activations/weights, far above the 126 MB L2"},
+                   "l2": "no explicit flush: one step streams >1 GB of activations/weights, far above the 50 MB L2"},
         "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": host_frames.numel() * 4,
                 "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / args.steps,
                 "input_copy": "every step's frame copied from pinned host memory inside the timed region, on a side "

@@ -1,5 +1,5 @@
 /*
- * msda_b200.h -- C ABI of the B200 (sm_100a) multi-scale deformable attention library
+ * msda_b200.h -- C ABI of the H100 (sm_90a) multi-scale deformable attention library
  * (libmsda_b200.so).  Plain pointers and sizes only; no torch types.
  *
  * Every entry point replaces a piece of the reference's compiled extension

@@ -1,5 +1,5 @@
 /*
- * tfb200_fused.h -- C ABI of the fused transformer-layer kernels in libmsda_b200.so (sm_100a).
+ * tfb200_fused.h -- C ABI of the fused transformer-layer kernels in libmsda_b200.so (sm_90a).
  *
  * These have NO counterpart in the reference's native code: the reference runs them as chains of PyTorch ops
  *   x = norm(x + dropout(branch))        src/trackformer/models/deformable_transformer.py:284-285, 291-292,
@@ -21,7 +21,7 @@ extern "C" {
 
 #define TFB200_E_NULLPTR (-1)
 #define TFB200_E_SHAPE   (-2)   /* C must be a multiple of 4, <= 512 (LayerNorm backward) / 1024 (forward, colsum) */
-#define TFB200_LN_MAX_CTAS 592  /* persistent grid: 148 SMs x 4 CTAs; also the row count of `partial_ws` */
+#define TFB200_LN_MAX_CTAS 528  /* persistent grid: 132 SMs x 4 CTAs; also the row count of `partial_ws` */
 
 /* number of CTAs (= rows of the [ctas][2][C] fp32 workspace the backward needs) for a problem of `rows` rows */
 int tfb200_ln_partial_ctas(int64_t rows);
@@ -110,8 +110,8 @@ int tfb200_frozen_bn_act_bwd_f32(const float* dy, const float* y, const float* s
 
 /* y[M][N] = act(x[M][K] . w[N][K]^T + bias[N])  -- the nn.Linear of the long-token projections / FFN
  * (ops/modules/ms_deform_attn.py:64,69,70,88; models/deformable_transformer.py:282-286) as ONE hand-written
- * tcgen05 kernel: TMA-staged 128x32 fp32 tiles, TF32 tensor-core products (tcgen05.mma kind::tf32), fp32
- * accumulation in TMEM, bias (+ optional ReLU) in the epilogue, TMA store.  All row-major, contiguous, 16-byte aligned.
+ * wgmma kernel: TMA-staged 128x32 fp32 tiles, TF32 tensor-core products (wgmma.mma_async .tf32), fp32
+ * accumulation in registers, bias (+ optional ReLU) in the epilogue, TMA store.  All row-major, contiguous, 16-byte aligned.
  * Requires N % 128 == 0 and K % 32 == 0 (tfb200_tf32_linear_supported); M is arbitrary.  bias may be NULL.
  * Returns -5 (unsupported) outside that domain: the caller keeps the library GEMM for those.                          */
 int tfb200_tf32_linear_supported(int64_t M, int N, int K);

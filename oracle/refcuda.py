@@ -1,6 +1,6 @@
 """ORACLE -- TEST INFRASTRUCTURE ONLY.  ctypes front-end of oracle/_ref/libmsda_refcuda.so: the reference's OWN CUDA
-kernels (ms_deform_im2col_cuda.cuh) compiled for sm_100a from the sources where they lie (oracle/Makefile `ref`,
-build container only).  GPU-vs-GPU parity checks and the "kernel to beat" timing use it; the product never does."""
+kernels (ms_deform_im2col_cuda.cuh) compiled for sm_90a from the reference sources (oracle/Makefile `ref`,
+only where those sources are present).  GPU-vs-GPU parity checks and the "kernel to beat" timing use it; the product never does."""
 from __future__ import annotations
 
 import ctypes

@@ -3,7 +3,7 @@
 // the include below; nothing from it is copied into this repository).  Built only in the build container
 // (`make -f oracle/Makefile ref` -> oracle/_ref/libmsda_refcuda.so, git-ignored, shipped to the GPU box by gpurun) and
 // used by tests/test_refcuda_gpu.py and tools/opbench.py as (a) a GPU-vs-GPU parity check against the real reference
-// kernels and (b) "the kernel to beat" on the same B200.
+// kernels and (b) "the kernel to beat" on the same GPU.
 //
 // The reference's host wrappers (ms_deform_attn_cuda.cu) depend on ATen; this file restates only their launch
 // sequence: forward = im2col kernel into a [L*P, N, Lq, M, D] `columns` buffer + sum over L*P (at::sum there,

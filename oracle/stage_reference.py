@@ -4,7 +4,7 @@ Stages the reference's Python model package and configs from /root/reference int
 ``baseline/_ref/`` so that they travel to the GPU box with the snapshot (the reference tree itself does not exist
 there).  Nothing is copied into the repository's history; the product never imports it.  Used by
 tools/ref_gpu_bench.py for (a) the zero-edit drop-in run -- the reference's own ``MSDeformAttn`` / ``DeformableDETR``
-classes on this repo's ``MultiScaleDeformableAttention`` extension -- and (b) the "reference on the same B200" arm
+classes on this repo's ``MultiScaleDeformableAttention`` extension -- and (b) the "reference on the same GPU" arm
 -- the same classes on the reference's own CUDA kernels (oracle/_ref).
 """
 from __future__ import annotations

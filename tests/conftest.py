@@ -1,7 +1,6 @@
 """pytest configuration: registers the ``gpu`` marker and shared fixtures.
 
-``-m "not gpu"`` runs in the CPU-only build container; ``-m gpu`` runs on a B200 box,
-where /root/reference does not exist -- GPU tests use only committed fixtures.
+``-m "not gpu"`` runs without a GPU; ``-m gpu`` runs on an H100.  Both use only committed fixtures.
 """
 import glob
 import os
@@ -18,7 +17,7 @@ GOLDEN_DIR = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 def golden_names(prefix="msda_"):

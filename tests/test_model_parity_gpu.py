@@ -1,4 +1,4 @@
-"""GPU model-level parity: the trackformer_b200 model on the real sm_100a kernels against golden outputs
+"""GPU model-level parity: the trackformer_b200 model on the real sm_90a kernels against golden outputs
 recorded from the reference classes on CPU (tests/golden/make_golden_model.py).
 
 Tolerance (BASELINE.json north_star): boxes / logits within 1e-3 relative of the reference; index
@@ -190,8 +190,8 @@ def test_train_step_c2_tf32(dev, tf32):
     print("tf32 gradients (max rel err, cosine):", rep)
     for k, (err, cos) in rep.items():
         # sampling-offset gradients are sums of DIFFERENCES of neighbouring value rows (the bilinear derivative), so a
-        # TF32 value projection (~5e-4 relative per element) shows up amplified there: measured on B200 cosine 0.9983,
-        # worst element 9 % of the largest gradient; every other tensor stays above 0.9998
+        # TF32 value projection (~5e-4 relative per element) shows up amplified there, hence
+        # the looser cosine bound for those tensors
         assert cos > (0.995 if "sampling_offsets" in k else 0.999), (k, err, cos)
 
 

@@ -1,4 +1,4 @@
-"""GPU parity tests of the MSDeformAttn hot path (run on the B200 box: ``pytest -m gpu``).
+"""GPU parity tests of the MSDeformAttn hot path (run on an H100: ``pytest -m gpu``).
 
 Every test goes through the product boundary -- the compiled module
 ``MultiScaleDeformableAttention`` / ``MSDeformAttnFunction`` (which call through the C ABI of

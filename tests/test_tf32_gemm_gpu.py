@@ -1,4 +1,4 @@
-"""The hand-written tcgen05 TF32 Linear (csrc/tf32_gemm.cu): forward (+bias, +ReLU), dgrad (MN-major weight operand),
+"""The hand-written wgmma TF32 Linear (csrc/tf32_gemm.cu): forward (+bias, +ReLU), dgrad (MN-major weight operand),
 split-token wgrad (TMA reduce-add) against fp64 products.  Tolerance: TF32 operands (10-bit mantissa, truncated by the
 tensor core) with fp32 accumulation -> ~1e-3 of the result scale, the same class as cuBLAS' TF32 kernels, whose error
 is printed next to ours."""
@@ -63,7 +63,7 @@ def test_unsupported_shapes_are_refused(op, cuda_device):
 
 
 def test_fused_linear_autograd_matches_library(cuda_device, monkeypatch):
-    """trackformer_b200.fused_linear.linear with the tcgen05 path on: outputs and all three gradients against F.linear"""
+    """trackformer_b200.fused_linear.linear with the wgmma path on: outputs and all three gradients against F.linear"""
     import trackformer_b200.fused_linear as fl
     monkeypatch.setattr(fl, "_TCGEN05", True)
     old = torch.backends.cuda.matmul.allow_tf32

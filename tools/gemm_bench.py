@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tools/gemm_bench.py -- the hand-written tcgen05 TF32 Linear (csrc/tf32_gemm.cu) against torch / cuBLAS.
+"""tools/gemm_bench.py -- the hand-written wgmma TF32 Linear (csrc/tf32_gemm.cu) against torch / cuBLAS.
 
 Checks values (TF32 tolerance against an fp64 product) and times both with CUDA events (L2 flushed between
 launches) on the long-token shapes of the C2 step.  Prints one JSON line per shape; --out writes the list.

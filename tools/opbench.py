@@ -134,7 +134,7 @@ def main():
     msda = ext.load()
     dev = torch.device("cuda:0")
     peak, peak_src = hbm_peak()
-    flush = torch.zeros(256 * 1024 * 1024 // 4, device=dev)       # 256 MB > 126 MB L2
+    flush = torch.zeros(256 * 1024 * 1024 // 4, device=dev)       # 256 MB > 50 MB L2
     results = []
     for name in args.cases.split(","):
         (value, shapes, loc, attn, gout), dims, fwd_b, bwd_b = make_case(name, dev)
@@ -176,7 +176,7 @@ def main():
                 results.append(r)
                 print(json.dumps(r), flush=True)
     msda.set_variant(0, 0)
-    # "the kernel to beat": the reference's own CUDA kernels compiled for sm_100a (oracle/_ref, test infrastructure)
+    # "the kernel to beat": the reference's own CUDA kernels compiled for sm_90a (oracle/_ref, test infrastructure)
     try:
         from oracle import refcuda
         have_ref = refcuda.available() and not args.once and args.ref

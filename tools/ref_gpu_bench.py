@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tools/ref_gpu_bench.py -- the REFERENCE's own model classes on the same B200 (test / measurement infrastructure).
+"""tools/ref_gpu_bench.py -- the REFERENCE's own model classes on the same GPU (test / measurement infrastructure).
 
 Runs the unmodified reference Python package staged under the git-ignored baseline/_ref/ (oracle/stage_reference.py)
 through its own training hot lines (src/trackformer/engine.py:126-151: model, SetCriterion with the scipy Hungarian
@@ -9,7 +9,7 @@ matcher, backward, clip_grad_norm_(0.1), AdamW), eagerly, as the reference runs,
                   the zero-edit drop-in route of INTEGRATION.md, executed on the GPU.  With --check the reference
                   model's outputs are compared with trackformer_b200's own model on the same weights and frame.
   --msda refcuda  the module is a thin shim over oracle/_ref/libmsda_refcuda.so, i.e. the reference's own CUDA kernels
-                  compiled for sm_100a: "the reference on the same B200" -- the honest GPU-vs-GPU denominator next to
+                  compiled for sm_90a: "the reference on the same GPU" -- the honest GPU-vs-GPU denominator next to
                   the CPU arm of bench.py.
 
 Prints one JSON line per run (frames/s of the C2 train step, 800x1333, batch 1, TF32 like bench.py).

@@ -1,4 +1,4 @@
-"""trackformer_b200 -- B200-native (sm_100a) implementation of TrackFormer's per-frame hot path:
+"""trackformer_b200 -- H100-native (sm_90a) implementation of TrackFormer's per-frame hot path:
 the Deformable-DETR encoder-decoder centred on the multi-scale deformable attention operator.
 
 Layout

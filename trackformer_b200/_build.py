@@ -6,7 +6,7 @@ Artefacts (git-ignored, shipped to the GPU box by gpurun):
 
 The reference builds its extension with a CUDAExtension and *no* -gencode flags
 (src/trackformer/models/ops/setup.py:34-39) and refuses to build without a visible GPU
-(:40-41); here nvcc cross-compiles for sm_100a explicitly, GPU or not.
+(:40-41); here nvcc cross-compiles for sm_90a (H100) explicitly, GPU or not.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_SO = os.path.join(HERE, "libmsda_b200.so")
 EXT_SO = os.path.join(HERE, "MultiScaleDeformableAttention.so")
 
-GENCODE = ["-gencode", "arch=compute_100a,code=sm_100a"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _nvcc() -> str:
@@ -51,7 +51,7 @@ def _run(cmd, verbose):
 def build_library(force: bool = False, verbose: bool = False) -> str:
     srcs = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith((".cu", ".cuh", ".h"))]
     srcs += _public_headers()
-    if not force and _newer(LIB_SO, srcs):
+    if not force and _newer(LIB_SO, [*srcs, __file__]):              # a change of the flags here rebuilds too
         return LIB_SO
     cu = [s for s in srcs if s.endswith(".cu")]
     _run([_nvcc(), "-O3", "-std=c++17", *GENCODE, "-lineinfo", "-Xcompiler", "-fPIC", "-shared",
@@ -63,7 +63,7 @@ def build_extension(force: bool = False, verbose: bool = False) -> str:
     build_library(False, verbose)
     src = os.path.join(CSRC, "msda_torch.cpp")
     hdrs = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith(".h")]
-    if not force and _newer(EXT_SO, [src, LIB_SO, *hdrs, *_public_headers()]):
+    if not force and _newer(EXT_SO, [src, LIB_SO, __file__, *hdrs, *_public_headers()]):
         return EXT_SO
     import torch
     from torch.utils import cpp_extension as ce

@@ -19,8 +19,8 @@ from .util import (accuracy, box_cxcywh_to_xyxy, generalized_box_iou, get_world_
 
 
 
-# SetCriterion losses (+ their backward) as fused device kernels (csrc/set_loss.cu); off until validated on a B200
-_FUSED_LOSS = os.environ.get("TFB200_FUSED_LOSS", "1") != "0"      # validated on B200: 67.5 -> 69.6 frames/s (profiles/r2_ab_call10.txt)
+# SetCriterion losses (+ their backward) as fused device kernels (csrc/set_loss.cu)
+_FUSED_LOSS = os.environ.get("TFB200_FUSED_LOSS", "1") != "0"
 
 
 class _SetLoss(torch.autograd.Function):

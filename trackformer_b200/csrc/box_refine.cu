@@ -1,4 +1,4 @@
-// boxes = sigmoid(delta + inverse_sigmoid(reference)) in one launch per direction (sm_100a).
+// boxes = sigmoid(delta + inverse_sigmoid(reference)) in one launch per direction (sm_90a).
 //
 // The reference refines its reference boxes after every decoder layer and again in the detection heads with a chain
 // of ~8 PyTorch ops per call -- clamp(0,1), clamp(min=eps), 1-x, clamp(min=eps), div, log, add, sigmoid

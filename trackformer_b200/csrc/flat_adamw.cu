@@ -1,4 +1,4 @@
-// Gradient clipping + AdamW over one flat fp32 parameter range in a single pass (sm_100a).
+// Gradient clipping + AdamW over one flat fp32 parameter range in a single pass (sm_90a).
 //
 // The reference step ends with clip_grad_norm_ and torch.optim.AdamW over ~600 parameter tensors
 // (src/trackformer/engine.py:147-151, src/train.py:118-119).  With every parameter, gradient and moment living in
@@ -70,7 +70,7 @@ extern "C" int tfb200_flat_adamw_f32(float* param, const float* grad, float* exp
   AdamArgs a{lr, beta1, beta2, eps, weight_decay, float(double(lr) / bc1), float(1.0 / sqrt(bc2)), max_norm};
   const int64_t npk = n >> 2;
   int64_t ctas = (npk + 255) / 256;
-  if (ctas > 148 * 8) ctas = 148 * 8;            // grid-stride over 8 CTAs per SM
+  if (ctas > 132 * 8) ctas = 132 * 8;            // grid-stride over 8 CTAs per SM
   if (ctas < 1) ctas = 1;
   flat_adamw_kernel<<<unsigned(ctas), 256, 0, cudaStream_t(stream)>>>(param, grad, exp_avg, exp_avg_sq, n,
                                                                       grad_norm_dev, a);

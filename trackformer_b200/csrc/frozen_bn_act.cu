@@ -1,4 +1,4 @@
-// Frozen batch-norm + (residual add) + ReLU for NHWC activations in one pass (sm_100a).
+// Frozen batch-norm + (residual add) + ReLU for NHWC activations in one pass (sm_90a).
 //
 // The reference backbone (torchvision ResNet-50 with FrozenBatchNorm2d, src/trackformer/models/backbone.py:19-55,
 // 98-100) runs  y = relu(x * scale[c] + shift[c] [+ identity])  as 2-3 separate elementwise passes after every one of
@@ -15,7 +15,7 @@
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kMaxCtas = 148 * 8;
+constexpr int kMaxCtas = 132 * 8;
 
 template <bool RELU, bool RES>
 __global__ void __launch_bounds__(kThreads)

@@ -1,10 +1,10 @@
-// Fused residual + dropout + LayerNorm for the transformer layers of the hot path (sm_100a).
+// Fused residual + dropout + LayerNorm for the transformer layers of the hot path (sm_90a).
 //
 // The reference's encoder/decoder layers compute   x = norm(x + dropout(branch))
 // (src/trackformer/models/deformable_transformer.py:291-292, 284-285, 370-371, 377-378, 360-361) as three
 // PyTorch ops forward (dropout, add, LayerNorm) and four backward (LayerNorm input grad, gamma/beta grad,
 // add, dropout grad).  On a C2 frame each of these is a pass over a [22223, 256] fp32 tensor (22.8 MB) and
-// PyTorch's LayerNorm backward alone takes ~180 us per call on B200.  These kernels do each direction in ONE
+// PyTorch's LayerNorm backward alone makes several passes over it.  These kernels do each direction in ONE
 // streaming pass (HBM-bound: forward reads x, branch, mask and writes s = x + drop(branch), y; backward reads
 // dy, s, mask and writes dx, dbranch) with a deterministic two-stage column reduction for dgamma / dbeta.
 //
@@ -345,7 +345,7 @@ relu_dropout_bwd_kernel(const float* __restrict__ gh, const float* __restrict__ 
 
 int grid_for(int64_t rows) {
   const int64_t need = (rows + kWarpsPerCta - 1) / kWarpsPerCta;
-  const int64_t cap = TFB200_LN_MAX_CTAS;          // persistent: 148 SMs x 4 resident CTAs
+  const int64_t cap = TFB200_LN_MAX_CTAS;          // persistent: 132 SMs x 4 resident CTAs
   return int(need < cap ? (need > 0 ? need : 1) : cap);
 }
 
@@ -484,7 +484,7 @@ int tfb200_relu_dropout_fwd_f32(const float* a, float* h, const int64_t* seed_de
   if (n < 0 || n % 4 != 0) return TFB200_E_SHAPE;
   if (n == 0) return 0;
   const int64_t n4 = n / 4;
-  const int grid = int(n4 / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int grid = int(n4 / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
   const uint32_t thresh = keep_threshold(keep_prob);
   relu_dropout_fwd_kernel<<<grid, 256, 0, cudaStream_t(stream)>>>(a, h, seed_dev, n4, training ? 1.f / keep_prob : 1.f,
                                                                   thresh, training);
@@ -498,7 +498,7 @@ int tfb200_relu_dropout_bwd_f32(const float* grad_h, const float* h, float* grad
   if (n < 0 || n % 4 != 0) return TFB200_E_SHAPE;
   if (n == 0) return 0;
   const int64_t n4 = n / 4;
-  const int grid = int(n4 / 256 < 148 * 16 ? (n4 + 255) / 256 : 148 * 16);
+  const int grid = int(n4 / 256 < 132 * 16 ? (n4 + 255) / 256 : 132 * 16);
   relu_dropout_bwd_kernel<<<grid, 256, 0, cudaStream_t(stream)>>>(grad_h, h, grad_a, n4, training ? 1.f / keep_prob : 1.f);
   msda_b200_count_launches(1);
   return int(cudaGetLastError());
@@ -604,7 +604,7 @@ sampling_prep_bwd_kernel(const float* __restrict__ grad_loc, const float* __rest
 
 int prep_grid(int64_t total) {
   const int64_t need = (total + 255) / 256;
-  return int(need < 148 * 16 ? need : 148 * 16);
+  return int(need < 132 * 16 ? need : 132 * 16);
 }
 
 }  // namespace

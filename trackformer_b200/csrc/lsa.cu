@@ -1,4 +1,4 @@
-// Device-side Hungarian matching for the set-prediction loss (sm_100a).
+// Device-side Hungarian matching for the set-prediction loss (sm_90a).
 //
 // The reference computes the matching cost on the GPU, copies it to the host and calls
 // scipy.optimize.linear_sum_assignment once per decoder layer (src/trackformer/models/matcher.py:104,127 -- six

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a multi-scale deformable attention kernels.
+// Shared device helpers for the sm_90a multi-scale deformable attention kernels.
 //
 // Semantics follow the reference CUDA op (timmeinhardt/trackformer,
 // src/trackformer/models/ops/src/cuda/ms_deform_im2col_cuda.cuh):

@@ -1,7 +1,7 @@
 // Kernels specialised for the shipped geometry: fp32, D = 32 channels per head (one head row of
 // `value` = 128 bytes = exactly one L1/L2 line), any M / L / P with L*P <= kMaxLP.
 //
-// What bounds these kernels (ncu, profiles/): every bilinear corner is a 128-byte row that has to
+// What bounds these kernels: every bilinear corner is a 128-byte row that has to
 // cross the SM's L1 data stage -- 4 wavefronts per warp-level LDG.128 -- so a C2 encoder call moves
 // 1.46 GB through L1 although only 80 MB are compulsory HBM traffic.  The design therefore minimises
 // every OTHER wavefront and instruction around those loads:
@@ -82,7 +82,7 @@ __device__ __forceinline__ void axis_window(float t, int size, int& b, float& wa
 // warp's four 8-lane groups -> the four queries makes the 4 rows touched by one warp-level LDG/RED belong to
 // NEIGHBOURING QUERIES OF ONE HEAD.  On the coarser levels neighbouring queries sample the same pixels, so
 // the LSU sees 1-2 distinct 128-byte lines per request instead of 4 (an L1 request costs ~2 cycles per
-// distinct line, profiles/).  Other head counts keep memory order.
+// distinct line).  Other head counts keep memory order.
 template <int STRIDE_CT>
 __device__ __forceinline__ int group_slot(int gl) {
   return STRIDE_CT == 256 ? ((gl & 3) * 8 + (gl >> 2)) : gl;

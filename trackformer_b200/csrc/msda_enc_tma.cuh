@@ -3,7 +3,7 @@
 // Reference semantics: ms_deform_im2col_cuda.cuh:165-237 (forward sampling kernel) -- identical taps, weights and zero
 // padding; only the data movement differs.
 //
-// What the measurements of the direct kernels say (DESIGN.md 3, profiles/): a C2 encoder call gathers 11.4 M corner
+// What the measurements of the direct kernels say : a C2 encoder call gathers 11.4 M corner
 // rows of 128 bytes (1.46 GB, 18x the compulsory bytes).  Through L1 a row costs ~2 cycles of the data stage no matter
 // how the request is shaped (92 us); cutting the rows with register-resident windows (msda_run*.cuh) made the direct
 // kernels latency bound instead (one window load per group in flight, L2 latency, little L1 left beside 41-49 KB of

@@ -41,15 +41,24 @@ inline void eb_fill_signs(EbSigns* t) {
     t->v[c] = make_float4(eb_dec_c(c), eb_dec_c(c >> 2), eb_dec_c(c >> 4), eb_dec_c(c >> 6));
 }
 
-__device__ __forceinline__ u64 fmul2(u64 a, u64 b) {
+// two-lane fp32 helpers on 64-bit register pairs: sm_90 has no packed fp32 arithmetic, so each lane is one IEEE op
+__device__ __forceinline__ float2 unpk2(u64 a) {
+  float2 r;
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(a));
+  return r;
+}
+__device__ __forceinline__ u64 pk2(float x, float y) {
   u64 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
+  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(x), "f"(y));
   return d;
 }
+__device__ __forceinline__ u64 fmul2(u64 a, u64 b) {
+  const float2 x = unpk2(a), y = unpk2(b);
+  return pk2(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y));
+}
 __device__ __forceinline__ u64 ffma2v(u64 a, u64 b, u64 c) {
-  u64 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  const float2 x = unpk2(a), y = unpk2(b), z = unpk2(c);
+  return pk2(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
 }
 __device__ __forceinline__ float hsum2(u64 v) {
   float a, b;
@@ -75,11 +84,8 @@ __device__ __forceinline__ void red2_if(const float* p, const u64 (&v)[2], bool 
 // acc = acc * keep + k * g  (keep = 0 right after the set was flushed, else 1; both lanes of the f32x2).  Arithmetic
 // instead of a select: ptxas turns a predicated mul / fma pair into both products plus two SELs per register pair.
 __device__ __forceinline__ void acc2(u64& acc, float k, u64 g, float keep) {
-  u64 kk, kp;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(kk) : "f"(k));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(kp) : "f"(keep));
-  const u64 t = fmul2(kk, g);
-  asm("fma.rn.f32x2 %0, %0, %1, %2;" : "+l"(acc) : "l"(kp), "l"(t));
+  const float2 a = unpk2(acc), v = unpk2(g);
+  acc = pk2(__fmaf_rn(a.x, keep, __fmul_rn(k, v.x)), __fmaf_rn(a.y, keep, __fmul_rn(k, v.y)));
 }
 
 // One sample slot of one level for one warp: the run of R queries, forward values + all three gradients.

@@ -1,4 +1,4 @@
-// libmsda_b200: hand-written sm_100a kernels for multi-scale deformable attention
+// libmsda_b200: hand-written sm_90a kernels for multi-scale deformable attention
 // (forward + fused backward) behind the C ABI declared in include/msda_b200.h.
 //
 // Replaces the reference's three kernels + host wrappers
@@ -258,14 +258,14 @@ static Family pick_family(int variant, int64_t groups, const struct Dims& d);
       value, shapes, loc, attn, gout, gval, gloc, gattn, d.S, d.M, d.D, d.L, d.Lq, d.P, groups)
 
 // Strip length (iterations of 32 groups) per CTA for the d32 kernels: keep at least ~2 waves of CTAs in
-// flight on the device's SMs (148 on a B200), but let big problems walk contiguous strips so neighbouring queries share L1 lines.
+// flight on the device's SMs (132 on an H100 SXM), but let big problems walk contiguous strips so neighbouring queries share L1 lines.
 static int pick_iters(int64_t ctas) {
   static std::atomic<int> sms{0};
   int n = sms.load(std::memory_order_relaxed);
   if (n == 0) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     sms.store(n, std::memory_order_relaxed);
   }
   const int64_t two_waves = int64_t(n) * 8 * 2;
@@ -290,12 +290,11 @@ static Family pick_family(int variant, int64_t groups, const Dims& d) {
   if (variant == 110) return Family::kWide;
   if (variant != 0) return Family::kD32;                    // the older tuning codes address the d32 kernels
   if (groups <= 32768) return Family::kWide;
-  // Measured on B200 (profiles/r2_opbench_v1.json, r2_opbench_v2.json): the run kernels cut the rows through L1 to
-  // ~0.3x but serialise one window load per group and need 41-49 KB of shared memory per CTA (little L1 left), and end
-  // up latency bound -- C2 encoder forward 121 us (run8) / 96 us (run4) / 106 us (run2) against 102 us for the
-  // 8-lane-group kernels, backward 286 / 228 vs 235 us.  They stay selectable (variants 100, 101, 120, 121).
-  // The multi-frame geometry (D = 36, C5 encoder call) is the exception: R = 4 runs take 256 us forward / 669 us backward
-  // against 275 us (nine-lane kernel) / 841 us (generic backward) -- profiles/r2_opbench_c5.json.
+  // The run kernels cut the rows through L1 to ~0.3x but serialise one window load per group and need 41-49 KB of
+  // shared memory per CTA (little L1 left), and end up latency bound at the C2 encoder geometry, so the 8-lane-group
+  // kernels serve it; the run kernels stay selectable (variants 100, 101, 120, 121).  The multi-frame geometry
+  // (D = 36, C5 encoder call) is the exception, where R = 4 runs beat the nine-lane / generic kernels.  This selection
+  // has not been re-timed on H100 (tools/opbench.py times every variant).
   if (run_ok && d.D == 36 && d.Lq >= 2048) return Family::kRun4;
   return Family::kD32;
 }
@@ -406,7 +405,7 @@ static int forward_impl(const T* value, const int64_t* shapes, const T* loc, con
       else if (d.M == 8 && tuning == 6) MSDA_FWD_D32(4, 4);
       else if (d.M == 8 && tuning == 7) MSDA_FWD_D32(8, 2);
       else if (d.M == 8 && tuning == 8) MSDA_FWD_D32(4, 1);
-      else if (d.M == 8) MSDA_FWD_D32(4, 4);          // measured best overall (profiles/): 64 registers, 4 CTAs/SM
+      else if (d.M == 8) MSDA_FWD_D32(4, 4);          // measured best overall: 64 registers, 4 CTAs/SM
 #undef MSDA_FWD_D32
       else {
         MSDA_ENSURE_SMEM((msda_fwd_d32_kernel<0>), smem);
@@ -576,7 +575,7 @@ static int backward_impl(const T* value, const int64_t* shapes, const T* loc, co
 // ---- measurement aid: what can the L1 data stage deliver for THIS access pattern? -------------------------------
 // Every warp issues LDG.128 requests shaped exactly like the gather's: 4 groups x 8 lanes, each group reading one
 // 128-byte row chosen pseudo-randomly from a table of `rows` rows (table small => L1 hits; 22.8 MB => L2 hits).
-// Nothing else happens, so bytes/time is the ceiling the MSDeformAttn gather can reach on this part (DESIGN.md 3).
+// Nothing else happens, so bytes/time is the ceiling the MSDeformAttn gather can reach on this part.
 __global__ void __launch_bounds__(256)
 l1_gather_probe_kernel(const float4* __restrict__ table, float4* __restrict__ sink, uint32_t rows, int iters) {
   const uint32_t gid = (blockIdx.x * 256u + threadIdx.x) >> 3;
@@ -882,8 +881,8 @@ int msda_b200_backward_enc_tiled_f32(const float* value, const int64_t* spatial_
   // kernel walks those levels from global memory, one L2 round trip per step, and its slowest CTAs are exactly these
   // (16 % of the kernel's time for 8 % of the samples, ncu).  Experiment: with the device copy of the level sizes at hand
   // they can go to the 8-lane-group kernel instead while the tile kernel keeps the level-0 tiles.
-  // Measured on B200 (C2 call): 220 us with the split against 216 us without -- the 8-lane-group kernel needs as long for
-  // that quarter of the queries as the tile kernel's slow CTAs, so the split is OFF unless asked for (variant 203).
+  // The 8-lane-group kernel needs about as long for that quarter of the queries as the tile kernel's slow CTAs, so the
+  // split did not pay and is OFF unless asked for (variant 203).
   const bool split = spatial_shapes_dev != nullptr && L > 1 && g_bwd_variant.load(std::memory_order_relaxed) == 203;
   if (split) {
     g.tiles_used = g.tile_begin[1];

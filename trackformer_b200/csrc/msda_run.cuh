@@ -1,7 +1,7 @@
 // "Run" kernels for fp32, D = 32 (128-byte head rows), large query sets (the encoder: Lq = S, raster order).
 //
 // Why: the gather is bound by L1 wavefronts (one per 128-byte corner row) and, in the backward, by the
-// L2 reduction units (one RED.128 per corner row) -- not by HBM (DESIGN.md 3).  In the encoder, consecutive
+// L2 reduction units (one RED.128 per corner row) -- not by HBM.  In the encoder, consecutive
 // queries are neighbouring pixels and their sampling windows on a level overlap: on the query's own level the
 // 2x2 window slides by one pixel per query (the right column becomes the left one), on the coarser levels it
 // mostly does not move at all.  So instead of giving a query's 16 samples to one 8-lane group (which reads

@@ -9,9 +9,8 @@
 //     prologue and its decisions are written back into the tap table: the bilinear weights already permuted into
 //     register-set order (A-top, B-top, A-bottom, B-bottom) and two 32-bit element offsets (column to load into set A,
 //     column to load into set B; kNoLoad = keep).  The hot loop has no state logic left.
-//   * FFMA2.  sm_100 has a packed two-lane fp32 FMA (PTX fma.rn.f32x2, SASS FFMA2 with a broadcast scalar operand):
-//     a weight times a 16-byte pack is 2 instructions instead of 4.  Each lane result is an IEEE fp32 FMA, so values
-//     equal the scalar form bit for bit.
+//   * Packed pairs.  Window values travel as 64-bit register pairs (two fp32 lanes); sm_90 has no packed fp32 FMA,
+//     so ffma2 issues one IEEE fp32 FMA per lane (the pair moves are register renames and cost no instruction).
 //   * lean addressing: unsigned 32-bit element offsets + one IMAD.WIDE.U32 per row address.
 //   * NS sample slots of a level walk the run INTERLEAVED (their windows live in separate registers): the loads of
 //     all NS slots of a step are issued before the first FMA of the step, so NS x 4 row loads are in flight per lane
@@ -32,9 +31,12 @@ __host__ __device__ inline int run2_entries(int R, int LP) { return 4 * R * kRun
 __host__ __device__ inline size_t fwd_run2_smem_bytes(int R, int LP) { return size_t(run2_entries(R, LP)) * (16 + 8); }
 
 __device__ __forceinline__ void ffma2(u64& acc, float w, u64 v) {
-  u64 ww;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(ww) : "f"(w));
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(ww), "l"(v));
+  float a0, a1, v0, v1;
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(a0), "=f"(a1) : "l"(acc));
+  asm("mov.b64 {%0, %1}, %2;" : "=f"(v0), "=f"(v1) : "l"(v));
+  a0 = __fmaf_rn(w, v0, a0);
+  a1 = __fmaf_rn(w, v1, a1);
+  asm("mov.b64 %0, {%1, %2};" : "=l"(acc) : "f"(a0), "f"(a1));
 }
 __device__ __forceinline__ void ldg2_if(u64& lo, u64& hi, const float* p, bool pred) {
   asm("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %3, 0;\n\t@p ld.global.nc.v2.b64 {%0, %1}, [%2];\n\t}"

@@ -347,7 +347,7 @@ at::Tensor colsum(const at::Tensor& x) {
   return out;
 }
 
-// y = act(x . w^T + bias) on the hand-written tcgen05 TF32 kernel (csrc/tf32_gemm.cu); x [..., K], w [N, K], bias [N] or None
+// y = act(x . w^T + bias) on the hand-written wgmma TF32 kernel (csrc/tf32_gemm.cu); x [..., K], w [N, K], bias [N] or None
 bool tf32_linear_supported(int64_t rows, int64_t n, int64_t k) { return tfb200_tf32_linear_supported(rows, int(n), int(k)) != 0; }
 
 at::Tensor tf32_linear(const at::Tensor& x, const at::Tensor& w, const c10::optional<at::Tensor>& bias, bool relu) {
@@ -780,7 +780,7 @@ std::vector<at::Tensor> add_dropout_layernorm_seeded_backward(const at::Tensor& 
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "B200 (sm_100a) multi-scale deformable attention; drop-in for the reference extension";
+  m.doc() = "H100 (sm_90a) multi-scale deformable attention; drop-in for the reference extension";
   m.def("ms_deform_attn_forward", &ms_deform_attn_forward, "ms_deform_attn_forward");
   m.def("ms_deform_attn_backward", &ms_deform_attn_backward, "ms_deform_attn_backward");
   // extras (not in the reference surface)

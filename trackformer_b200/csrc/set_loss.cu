@@ -1,4 +1,4 @@
-// SetCriterion on the device in three launches (sm_100a): matching cost, loss values + unit gradients, backward.
+// SetCriterion on the device in three launches (sm_90a): matching cost, loss values + unit gradients, backward.
 //
 // The reference evaluates the Hungarian cost matrix and the focal / L1 / GIoU losses of the six decoder layers as
 // chains of small PyTorch ops (src/trackformer/models/matcher.py:60-100, models/detr.py:213-328, util/misc.py:540-571,
@@ -12,7 +12,7 @@
 //   set_loss_final  one CTA per layer: fixed-order sums -> loss_ce / loss_bbox / loss_giou / cardinality_error (+ the
 //                   class error of the last layer), all divided by the device-resident normaliser num_boxes
 //   set_loss_bwd    grad_logits / grad_boxes from the three incoming gradient vectors [layers]
-// Gradient formulas verified against autograd (fp64) -- see DESIGN.md; torch's min / max / clamp subgradient
+// Gradient formulas verified against autograd (fp64); torch's min / max / clamp subgradient
 // conventions are kept (ties are measure-zero).
 #include <cuda_runtime.h>
 #include <stdint.h>

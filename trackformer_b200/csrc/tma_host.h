@@ -13,8 +13,8 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 // cuTensorMapEncodeTiled is a DRIVER call: it fails with CUDA_ERROR_INVALID_CONTEXT on a thread that has not touched
-// the runtime yet (PyTorch's autograd workers: the first CUDA work of a backward node may be our encode, measured on
-// B200 as error code -7 from tf32_linear_dgrad).  Binding the device's primary context once per thread fixes that.
+// the runtime yet (PyTorch's autograd workers: the first CUDA work of a backward node may be our encode, seen as
+// error code -7 from tf32_linear_dgrad).  Binding the device's primary context once per thread fixes that.
 inline void bind_primary_context_once() {
   thread_local bool bound = false;
   if (!bound) {

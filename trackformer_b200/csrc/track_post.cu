@@ -1,4 +1,4 @@
-// Detection post-processing for the online tracker in one launch (sm_100a).
+// Detection post-processing for the online tracker in one launch (sm_90a).
 //
 // The reference turns the decoder outputs into per-query detections with a chain of ~8 PyTorch ops
 // (src/trackformer/models/deformable_detr.py:286-334: sigmoid, max over classes, cxcywh -> xyxy, scale by the image

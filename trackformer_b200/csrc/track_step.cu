@@ -1,4 +1,4 @@
-// Tracker.step bookkeeping on the device (sm_100a): one CTA runs tfb200_track::ts_step (track_step_core.h) -- every
+// Tracker.step bookkeeping on the device (sm_90a): one CTA runs tfb200_track::ts_step (track_step_core.h) -- every
 // threshold, both NMS passes, public-detection gating, ReID and the result rows of src/trackformer/models/tracker.py:
 // 266-548 -- so a tracked frame costs one launch after the detector and one small device->host copy of the results,
 // instead of the reference's several .cpu() synchronisations per track per frame.

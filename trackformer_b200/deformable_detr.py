@@ -1,4 +1,4 @@
-"""Deformable-DETR detector shell around the B200 transformer.
+"""Deformable-DETR detector shell around the H100 transformer.
 
 Mirror of ``DETR`` (constructor state only: src/trackformer/models/detr.py:17-54), ``MLP`` (:493-507) and
 ``DeformableDETR`` (src/trackformer/models/deformable_detr.py:29-283) with the same forward signature

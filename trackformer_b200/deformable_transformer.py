@@ -1,4 +1,4 @@
-"""Deformable transformer (6 encoder + 6 decoder layers) on the B200 MSDeformAttn kernels.
+"""Deformable transformer (6 encoder + 6 decoder layers) on the H100 MSDeformAttn kernels.
 
 Mirror of src/trackformer/models/deformable_transformer.py (one-stage path, which is what every shipped
 config uses -- cfgs/train_deformable.yaml sets ``with_box_refine: true`` and leaves ``two_stage: false``):

@@ -1,4 +1,4 @@
-"""Linear layers and the FFN activation of the encoder with fused sm_100a epilogue kernels.
+"""Linear layers and the FFN activation of the encoder with fused sm_90a epilogue kernels.
 
 * ``linear(x, weight, bias)`` -- ``F.linear`` whose backward computes the bias gradient with the library's
   streaming column-sum kernel (one HBM-bound pass, deterministic) instead of PyTorch's generic reduction
@@ -30,13 +30,12 @@ def weight_grad(gy2: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
     """dW = gy2^T @ x2 for a long token axis ([22223, C] operands at the benchmark size).
 
     The product is a small [c_out, c_in] tile grid reduced over tens of thousands of rows; the library GEMM does not
-    split that reduction and runs 16-64 CTAs on a 148-SM part (38 us for 256 x 256 x 22223, 76 TFLOP/s).  Splitting
+    split that reduction and runs 16-64 CTAs on a 132-SM part.  Splitting
     the token axis into `s` slabs turns it into one batched GEMM with s x as many CTAs plus a [s, c_out, c_in] sum:
     same products, fp32 accumulation, only the summation order over tokens changes.
 
-    Measured (tools/wgrad_bench.py, cold L2): 44 -> 32 us for 256 x 256, 55 -> 36 us for 384 x 256; but inside the
-    replayed training step, where the operands were just written and sit in the 126 MB L2, the three launches cost
-    more than the split saves (16.31 ms/step without vs 16.71 ms with), so it is OFF unless TFB200_WGRAD_SPLITK=1."""
+    It is OFF unless TFB200_WGRAD_SPLITK=1: inside the replayed training step the operands were just written and sit
+    in L2, and the three launches cost more than the split saves (tools/wgrad_bench.py times both)."""
     k, c_out = gy2.shape
     c_in = x2.shape[1]
     tiles = -(-c_out // 128) * -(-c_in // 128)
@@ -52,18 +51,16 @@ def weight_grad(gy2: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
     return gw
 
 
-# Forward products of the long-token Linears on the hand-written tcgen05 kernel (csrc/tf32_gemm.cu) whenever TF32
+# Forward products of the long-token Linears on the hand-written wgmma kernel (csrc/tf32_gemm.cu) whenever TF32
 # tensor-core math is allowed (torch.backends.cuda.matmul.allow_tf32 -- the benchmark setting; strict-fp32 runs keep the
 # library's fp32 GEMM).  TFB200_TCGEN05_LINEAR=0 switches it off (A/B timing).
 _TCGEN05 = os.environ.get("TFB200_TCGEN05_LINEAR", "1") != "0"
 
 
-# Which of the three products run on it ("f" forward, "d" dgrad, "w" wgrad).  Measured on B200 (tools/gemm_bench.py,
-# profiles/r2_gemm_bench.json; one-call A/B of the whole step, profiles/r2_ab_call10.txt): the split-token wgrad beats
-# the library 1.3-2x (23.5 vs 44 us for 256 x 256 x 22223, 27.6 vs 56 us for 384 x 256) -- the library runs that
-# product on 8-32 CTAs; forward and dgrad are on par for N = 256 / 384 and ~1.3x slower for the 1024-wide FFN products
-# (128 x 128 tiles leave a 2.35-wave tail and re-stage W per tile).  Step: 67.5 -> 70.8 frames/s with "w", 69.8 with
-# "dw", 69.2 with "fdw".  Default: the product where the hand-written kernel wins.
+# Which of the three products run on it ("f" forward, "d" dgrad, "w" wgrad).  Measured on an H100 80GB HBM3 (400 W power
+# limit, tools/gemm_bench.py): the split-token wgrad is within 1-7 % of the library (36.4 vs 35.3 us for
+# 256 x 256 x 22223, 42.4 vs 39.6 us for 384 x 256); forward and dgrad are on par for N = 256 / 384 and up to 1.5x slower
+# for the 1024-wide FFN products.  Default: only the wgrad runs on the hand-written kernel.
 _TCGEN05_PARTS = os.environ.get("TFB200_TCGEN05_PARTS", "w")
 
 

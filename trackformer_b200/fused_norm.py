@@ -1,4 +1,4 @@
-"""``x = LayerNorm(x + dropout(branch))`` as one fused sm_100a kernel per direction.
+"""``x = LayerNorm(x + dropout(branch))`` as one fused sm_90a kernel per direction.
 
 Replaces the three-op forward / four-op backward chain the reference's transformer layers execute for every
 residual connection (src/trackformer/models/deformable_transformer.py:284-285, 291-292, 360-361, 370-371,

@@ -17,8 +17,8 @@ from torch import nn
 
 from .util import box_cxcywh_to_xyxy, generalized_box_iou
 
-# matching cost and SetCriterion losses as fused device kernels (csrc/set_loss.cu); off until validated on a B200
-_FUSED_LOSS = os.environ.get("TFB200_FUSED_LOSS", "1") != "0"      # validated on B200: 67.5 -> 69.6 frames/s (profiles/r2_ab_call10.txt)
+# matching cost and SetCriterion losses as fused device kernels (csrc/set_loss.cu)
+_FUSED_LOSS = os.environ.get("TFB200_FUSED_LOSS", "1") != "0"
 
 
 class HungarianMatcher(nn.Module):

@@ -1,4 +1,4 @@
-"""Autograd binding of the B200 MSDeformAttn kernels.
+"""Autograd binding of the H100 MSDeformAttn kernels.
 
 Mirror of the reference's ``MSDeformAttnFunction``
 (src/trackformer/models/ops/functions/ms_deform_attn_func.py:14-31): same ``apply`` signature
@@ -78,8 +78,8 @@ def _backward(ctx, grad_output, hw):
 
 # Which forward kernel serves an encoder call (queries == pixels): "tile" = the TMA-staged tile kernel
 # (csrc/msda_enc_tma.cuh), "direct" = the 8-lane-group kernel.  Which one is faster depends on how compact the sampling
-# pattern of neighbouring queries is (measured on B200, C2 encoder call: the grid pattern of a freshly initialised model
-# 82 vs 103 us, +-0.5 px of per-sample jitter 116 vs 106 us, uniformly random locations 224 vs 107 us), so in "auto"
+# pattern of neighbouring queries is (the tile kernel wins on the grid pattern of a freshly initialised model and loses
+# once the locations scatter), so in "auto"
 # mode the first eager call of a geometry times both on the data at hand and the winner is kept for that geometry.
 import os as _os
 
@@ -115,8 +115,7 @@ def encoder_kernel_choice(msda, value, shapes, loc, attn, hw, step):
 
 
 def encoder_backward_choice(msda, value, shapes, loc, attn, grad_out, hw, step):
-    """Same one-time measurement for the backward (C2 encoder call on B200: grid pattern 218 vs 235 us, +-0.5 px jitter
-    302 vs 245 us)."""
+    """Same one-time measurement for the backward."""
     if _TILED_ENC_BWD in ("0", "1"):
         return "tile" if _TILED_ENC_BWD == "1" else "direct"
     key = (tuple(value.shape), tuple(hw), value.device.index)

@@ -1,4 +1,4 @@
-"""``MSDeformAttn`` -- the multi-scale deformable attention layer on the B200 kernels.
+"""``MSDeformAttn`` -- the multi-scale deformable attention layer on the H100 kernels.
 
 Mirror of the reference module (src/trackformer/models/ops/modules/ms_deform_attn.py:15-89):
 same constructor, same sub-module names (``sampling_offsets``, ``attention_weights``, ``value_proj``,
@@ -24,7 +24,7 @@ from .fused_linear import linear as fused_linear
 from .msda_function import (MSDeformAttnEncFunction, MSDeformAttnEncFusedFunction, MSDeformAttnFunction,
                             MSDeformAttnFusedFunction, encoder_fused_choice)
 
-# fold sampling_prep into the MSDeformAttn kernels (csrc/msda_run.cuh PREP variants); off until validated on a B200
+# fold sampling_prep into the MSDeformAttn kernels (csrc/msda_run.cuh PREP variants)
 _FUSED_PREP = os.environ.get("TFB200_FUSED_PREP", "0") != "0"
 
 # the 8 compass directions the reference seeds the per-head offset bias with (ms_deform_attn.py:36)

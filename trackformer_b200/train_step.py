@@ -1,6 +1,6 @@
 """One training step of the detection hot path, replayed from CUDA graphs.
 
-This is the B200-side counterpart of the six hot lines of the reference's training loop
+This is the GPU-side counterpart of the six hot lines of the reference's training loop
 (src/trackformer/engine.py:126-151):
 
     outputs = model(samples, targets); loss_dict = criterion(outputs, targets); losses = sum(w_k * loss_k)
@@ -8,8 +8,8 @@ This is the B200-side counterpart of the six hot lines of the reference's traini
 
 plus the gradient all-reduce the reference gets from DistributedDataParallel (src/train.py:86-89).
 
-Why graphs: an eager PyTorch step of this model issues ~5000 small kernels and is host-bound (58 ms/step
-measured on a B200 box although the kernels themselves need < 20 ms).  The model forward and its
+Why graphs: an eager PyTorch step of this model issues ~5000 small kernels and is host-bound (the launch
+overhead exceeds the kernels' own run time).  The model forward and its
 backward are static-shape, sync-free programs, so they are captured once (``torch.cuda.CUDAGraph``) and
 replayed -- two graph launches instead of thousands of kernel launches.  The backward graph also contains the
 accumulation into the gradient buffer, so nothing per-parameter runs eagerly.  Between the two sits what cannot be captured: the Hungarian matching (scipy on the host, like the
