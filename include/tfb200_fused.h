@@ -218,6 +218,49 @@ typedef struct TfbTrackStepArgs {
 
 int tfb200_track_step_f32(const TfbTrackStepArgs* args, void* stream);
 
+/* Segmentation mask head between its convolutions, and its loss (csrc/mask_head.cu; reference
+ * models/detr_segmentation.py:111-216, models/detr.py:330-357).  Per-query maps are channels-last [N][HW][C] with
+ * N = images * per_image; an operand "per image" is [N / per_image][...] and is broadcast over that image's queries
+ * instead of being expanded.  Reductions over queries and samples run in a fixed order (no float atomics).
+ *
+ * mask_attn: w [B][Q][heads][HW] = softmax over HW of scale * q . k, -inf where pad (MHAttentionMap, head width 32).
+ *   q [B][Q][heads*32], k [B][HW][heads*32] token-major, pad [B][HW] bool or NULL.  q, k (and dk) must be
+ *   16-byte aligned, else TFB200_E_SHAPE.  backward: dq, dk from dw; ds_ws [B][Q][heads][HW] scratch.            */
+int tfb200_mask_attn_fwd_f32(const float* q, const float* k, const uint8_t* pad, float* w, int B, int Q, int HW,
+                             int heads, float scale, void* stream);
+int tfb200_mask_attn_bwd_f32(const float* q, const float* k, const float* w, const float* dw, float* ds_ws, float* dq,
+                             float* dk, int B, int Q, int HW, int heads, float scale, void* stream);
+/* group_norm_relu: y = relu(GroupNorm_groups(x + addend) * gamma + beta), addend [N / per_image][HW][C] or NULL;
+ * mean / rstd [N][groups] are saved for the backward.  C / groups <= 256.  backward: dx, daddend (summed over each
+ * image's queries; required when addend is given), daffine [2][C] = {dgamma, dbeta}; partial_ws [N][2][C] scratch. */
+int tfb200_group_norm_relu_fwd_f32(const float* x, const float* addend, const float* gamma, const float* beta, float* y,
+                                   float* mean, float* rstd, int N, int per_image, int64_t HW, int C, int groups,
+                                   float eps, void* stream);
+int tfb200_group_norm_relu_bwd_f32(const float* dy, const float* x, const float* addend, const float* y,
+                                   const float* gamma, const float* mean, const float* rstd, float* dx, float* daddend,
+                                   float* daffine, float* partial_ws, int N, int per_image, int64_t HW, int C,
+                                   int groups, void* stream);
+/* upsample_add: out [N][Ho][Wo][C] = a[n / per_image] + x[n] nearest-upsampled from [Hi][Wi] (F.interpolate's
+ * nearest rule).  backward: dx [N][Hi][Wi][C] (block sums) and da [N / per_image][Ho][Wo][C] (sum over queries).    */
+int tfb200_upsample_add_fwd_f32(const float* x, const float* a, float* out, int N, int per_image, int Hi, int Wi,
+                                int Ho, int Wo, int C, void* stream);
+int tfb200_upsample_add_bwd_f32(const float* dout, float* dx, float* da, int N, int per_image, int Hi, int Wi, int Ho,
+                                int Wo, int C, void* stream);
+/* mask_loss: M matched pairs (logits row src[m] of [R][h][w], target mask tgt[m] of [T][Ht][Wt] bool).  The logits
+ * are sampled bilinearly (align_corners=False) at every target pixel on the fly; out2 = {sigmoid focal loss (mean
+ * over pixels), dice} summed over pairs and divided by the device scalar *num_boxes.  M == 0 gives zeros.
+ * stats [M][4] are saved for the backward; partial_ws [M][tfb200_mask_loss_partial_chunks(Ht, Wt)][4] scratch.
+ * backward: grad_logits [R][h][w] (zero outside the matched rows) from g2 = {dL/dloss_mask, dL/dloss_dice}.
+ * Precondition: src holds no row twice (a one-to-one matching guarantees it); each matched row's gradient is written,
+ * not accumulated.                                                                                                */
+int tfb200_mask_loss_partial_chunks(int Ht, int Wt);
+int tfb200_mask_loss_fwd_f32(const float* logits, const int64_t* src, const uint8_t* tgt_masks, const int64_t* tgt,
+                             const float* num_boxes, float* stats, float* partial_ws, float* out2, int M, int h, int w,
+                             int Ht, int Wt, float alpha, float gamma, void* stream);
+int tfb200_mask_loss_bwd_f32(const float* logits, const int64_t* src, const uint8_t* tgt_masks, const int64_t* tgt,
+                             const float* stats, const float* num_boxes, const float* g2, float* grad_logits, int R,
+                             int M, int h, int w, int Ht, int Wt, float alpha, float gamma, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

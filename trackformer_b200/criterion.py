@@ -4,7 +4,9 @@ Mirror of ``SetCriterion`` (src/trackformer/models/detr.py:139-443) for the loss
 TrackFormer configs use -- ``labels`` (sigmoid focal or weighted cross-entropy), ``boxes`` (L1 + GIoU) and
 ``cardinality`` (logging only) -- applied to the last decoder layer and to every auxiliary layer with its own
 Hungarian matching, normalised by the world-averaged number of boxes (one scalar all-reduce, :399-401).
-Mask losses belong to the segmentation heads, which are outside the hot path.
+``masks`` (sigmoid focal + dice on the bilinearly upsampled mask logits, :330-357) applies to the last layer only;
+on CUDA fp32 it is csrc/mask_head.cu, which samples the low-resolution logits at every target pixel on the fly
+instead of materialising the upsampled masks.
 """
 from __future__ import annotations
 
@@ -14,8 +16,61 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .util import (accuracy, box_cxcywh_to_xyxy, generalized_box_iou, get_world_size,
+from .util import (accuracy, box_cxcywh_to_xyxy, dice_loss, generalized_box_iou, get_world_size,
                    is_dist_avail_and_initialized, paired_giou, sigmoid_focal_loss)
+
+_MASK_ALPHA, _MASK_GAMMA = 0.25, 2.0          # loss_masks uses sigmoid_focal_loss's defaults (detr.py:353)
+
+
+class _MaskLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, src, tgt_masks, tgt, num_boxes):
+        from . import ext
+        out, stats = ext.load().mask_loss_forward(logits, src, tgt_masks, tgt, num_boxes, _MASK_ALPHA, _MASK_GAMMA)
+        ctx.save_for_backward(logits, src, tgt_masks, tgt, stats, num_boxes)
+        return out[0], out[1]
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_mask, g_dice):
+        from . import ext
+        logits, src, tgt_masks, tgt, stats, num_boxes = ctx.saved_tensors
+        g2 = torch.stack([g_mask, g_dice]).float()
+        grad = ext.load().mask_loss_backward(logits, src, tgt_masks, tgt, stats, num_boxes, g2, _MASK_ALPHA, _MASK_GAMMA)
+        return grad, None, None, None, None
+
+
+def _padded_target_masks(targets, device):
+    """All target masks of the batch as one [T, Hmax, Wmax] bool tensor, zero-padded to the largest image
+    (nested_tensor_from_tensor_list of detr.py:343, indexed by global box number instead of (image, box))."""
+    masks = [t["masks"] for t in targets]
+    h = max(m.shape[-2] for m in masks)
+    w = max(m.shape[-1] for m in masks)
+    out = torch.zeros((sum(len(m) for m in masks), h, w), dtype=torch.bool, device=device)
+    ofs = 0
+    for m in masks:
+        out[ofs:ofs + len(m), :m.shape[-2], :m.shape[-1]] = m.to(device=device, dtype=torch.bool)
+        ofs += len(m)
+    return out
+
+
+def mask_losses(pred_masks, src, tgt, targets, num_boxes):
+    """loss_mask / loss_dice of the matched pairs: row ``src[i]`` of ``pred_masks.flatten(0, 1)`` against global target
+    mask ``tgt[i]``.  Padding pixels count, as in the reference; no pairs give zero losses."""
+    dev = pred_masks.device
+    tmasks = _padded_target_masks(targets, dev)
+    src, tgt = src.to(dev), tgt.to(dev)
+    logits = pred_masks.flatten(0, 1)
+    if pred_masks.is_cuda and pred_masks.dtype == torch.float32:
+        nb = num_boxes if torch.is_tensor(num_boxes) else torch.tensor(float(num_boxes))
+        nb = nb.to(dev, torch.float32).reshape(1)
+        loss_mask, loss_dice = _MaskLoss.apply(logits.contiguous(), src, tmasks, tgt, nb)
+        return {"loss_mask": loss_mask, "loss_dice": loss_dice}
+    sm = F.interpolate(logits[src][:, None], size=tmasks.shape[-2:], mode="bilinear", align_corners=False)
+    sm = sm[:, 0].flatten(1)
+    tm = tmasks[tgt].flatten(1).to(sm)
+    return {"loss_mask": sigmoid_focal_loss(sm, tm, num_boxes, _MASK_ALPHA, _MASK_GAMMA),
+            "loss_dice": dice_loss(sm, tm, num_boxes)}
 
 
 
@@ -131,9 +186,19 @@ class SetCriterion(nn.Module):
         giou = 1 - torch.diag(generalized_box_iou(box_cxcywh_to_xyxy(src), box_cxcywh_to_xyxy(tgt)))
         return {"loss_bbox": l1.sum() / num_boxes, "loss_giou": giou.sum() / num_boxes}
 
+    def loss_masks(self, outputs, targets, indices, num_boxes):
+        assert "pred_masks" in outputs
+        n_q, dev = outputs["pred_masks"].shape[1], outputs["pred_masks"].device
+        offsets = [0]
+        for t in targets:
+            offsets.append(offsets[-1] + len(t["masks"]))
+        src = torch.cat([s.to(dev) + b * n_q for b, (s, _) in enumerate(indices)])
+        tgt = torch.cat([j.to(dev) + offsets[b] for b, (_, j) in enumerate(indices)])
+        return mask_losses(outputs["pred_masks"], src, tgt, targets, num_boxes)
+
     def get_loss(self, loss, outputs, targets, indices, num_boxes, **kwargs):
         table = {"labels": self.loss_labels_focal if self.focal_loss else self.loss_labels,
-                 "cardinality": self.loss_cardinality, "boxes": self.loss_boxes}
+                 "cardinality": self.loss_cardinality, "boxes": self.loss_boxes, "masks": self.loss_masks}
         assert loss in table, f"do you really want to compute {loss} loss?"
         return table[loss](outputs, targets, indices, num_boxes, **kwargs)
 
@@ -219,19 +284,23 @@ class SetCriterion(nn.Module):
         losses.stacked = (ce, l1, gi)
         return losses
 
-    def forward_stacked(self, logits, boxes, targets, num_boxes=None):
+    def forward_stacked(self, logits, boxes, targets, num_boxes=None, pred_masks=None):
         """Same losses as ``forward`` for a detector whose K decoder layers arrive stacked --
         ``logits [K,B,Q,C]``, ``boxes [K,B,Q,4]``, last layer = final prediction -- computed in ONE pass over
         all layers instead of K passes (the reference loops, detr.py:404-424): one Hungarian transfer, one focal
         loss, one L1/GIoU evaluation.  Keys and values equal ``forward`` on the equivalent dict (up to fp32
-        summation order); falls back to it for the cases that need per-layer bookkeeping."""
+        summation order); falls back to it for the cases that need per-layer bookkeeping.  With the ``masks`` loss,
+        ``pred_masks [B,Q,h,w]`` of the last layer is scored against the last layer's matching."""
         k, bs, nq, _ = logits.shape
         layers = [{"pred_logits": logits[i], "pred_boxes": boxes[i]} for i in range(k)]
-        special = (not self.focal_loss or set(self.losses) != {"labels", "boxes", "cardinality"}
+        with_masks = "masks" in self.losses
+        special = (not self.focal_loss or set(self.losses) - {"masks"} != {"labels", "boxes", "cardinality"}
                    or any("track_query_match_ids" in t for t in targets) or not hasattr(self.matcher, "match_layers"))
         sizes = [len(t["labels"]) for t in targets]
         if special or min(sizes) == 0 or max(sizes) > nq:
             out = dict(layers[-1])
+            if with_masks:
+                out["pred_masks"] = pred_masks
             out["aux_outputs"] = layers[:-1]
             return self.forward(out, targets, num_boxes)
 
@@ -267,8 +336,14 @@ class SetCriterion(nn.Module):
             idx = torch.stack([lay, bat, src, tgt]).to(dev, non_blocking=True)
             lay, bat, src, tgt = idx[0], idx[1], idx[2], idx[3]
             n_gt = torch.as_tensor(sizes, device=dev, dtype=torch.float)
+        if with_masks:
+            last = slice((k - 1) * per_layer, None)
+            masks = mask_losses(pred_masks, bat[last] * nq + src[last], tgt[last], targets, num_boxes)
         if device_match is not None and _FUSED_LOSS and logits.dtype == torch.float32:
-            return self._fused_losses(logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes)
+            losses = self._fused_losses(logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes)
+            if with_masks:
+                losses.update(masks)
+            return losses
         gt_labels = torch.cat([t["labels"] for t in targets])[tgt]
         gt_boxes = torch.cat([t["boxes"] for t in targets])[tgt]
 
@@ -306,4 +381,6 @@ class SetCriterion(nn.Module):
             losses[f"loss_giou_{i}"] = loss_giou[i]
             losses[f"cardinality_error_{i}"] = card[i]
         losses.stacked = (loss_ce, loss_bbox, loss_giou)
+        if with_masks:
+            losses.update(masks)
         return losses

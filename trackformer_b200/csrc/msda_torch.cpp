@@ -779,6 +779,202 @@ std::vector<at::Tensor> add_dropout_layernorm_seeded_backward(const at::Tensor& 
   return {dx, db, dgamma, dbeta};
 }
 
+// ---- segmentation mask head (csrc/mask_head.cu) ----
+static void check_f32(const at::Tensor& t, const char* what) {
+  TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kFloat, what, ": fp32 CUDA tensor required (no CPU path)");
+}
+
+static void check_nhwc(const at::Tensor& t, const char* what) {
+  check_f32(t, what);
+  TORCH_CHECK(t.dim() == 4 && t.is_contiguous(at::MemoryFormat::ChannelsLast), what,
+              ": [N, C, H, W] channels-last contiguous tensor required");
+}
+
+static at::Tensor empty_nhwc(at::IntArrayRef sizes, const at::Tensor& like) {
+  return at::empty(sizes, like.options().memory_format(at::MemoryFormat::ChannelsLast));
+}
+
+static void raise_rc(int rc, const char* what) { TORCH_CHECK(rc == 0, what, " failed (code ", rc, ")"); }
+
+// q [B, Q, heads*32], k [B, HW, heads*32], pad [B, HW] bool or None -> w [B, Q, heads, HW]
+at::Tensor mask_attn_forward(const at::Tensor& q, const at::Tensor& k, const c10::optional<at::Tensor>& pad, int64_t heads,
+                             double scale) {
+  check_f32(q, "mask_attn q");
+  check_f32(k, "mask_attn k");
+  TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && heads > 0 && q.size(2) == heads * 32 && k.size(2) == q.size(2) &&
+              k.size(0) == q.size(0) && k.size(1) > 0, "mask_attn: q [B, Q, heads*32], k [B, HW, heads*32]");
+  const at::Tensor qc = q.contiguous(), kc = k.contiguous();
+  TORCH_CHECK(reinterpret_cast<uintptr_t>(qc.data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(kc.data_ptr()) % 16 == 0,
+              "mask_attn: q and k must be 16-byte aligned");
+  const int B = int(q.size(0)), Q = int(q.size(1)), HW = int(k.size(1));
+  const uint8_t* pp = nullptr;
+  at::Tensor pc;
+  if (pad.has_value() && pad->defined()) {
+    pc = pad->contiguous();
+    TORCH_CHECK(pc.is_cuda() && pc.element_size() == 1 && pc.numel() == int64_t(B) * HW, "mask_attn: pad must be a bool [B, HW] CUDA tensor");
+    pp = reinterpret_cast<const uint8_t*>(pc.data_ptr());
+  }
+  const c10::cuda::CUDAGuard guard(q.device());
+  at::Tensor w = at::empty({B, Q, heads, HW}, qc.options());
+  raise_rc(tfb200_mask_attn_fwd_f32(qc.data_ptr<float>(), kc.data_ptr<float>(), pp, w.data_ptr<float>(), B, Q, HW,
+                                    int(heads), float(scale), c10::cuda::getCurrentCUDAStream().stream()),
+           "mask_attn_forward");
+  return w;
+}
+
+std::vector<at::Tensor> mask_attn_backward(const at::Tensor& q, const at::Tensor& k, const at::Tensor& w,
+                                           const at::Tensor& dw, double scale) {
+  check_f32(dw, "mask_attn dw");
+  TORCH_CHECK(w.dim() == 4 && dw.sizes() == w.sizes() && q.is_contiguous() && k.is_contiguous() && w.is_contiguous(),
+              "mask_attn_backward: saved tensors and dw [B, Q, heads, HW]");
+  const int B = int(w.size(0)), Q = int(w.size(1)), heads = int(w.size(2)), HW = int(w.size(3));
+  const at::Tensor dwc = dw.contiguous();
+  const c10::cuda::CUDAGuard guard(w.device());
+  at::Tensor ds = at::empty_like(w), dq = at::empty_like(q), dk = at::empty_like(k);
+  raise_rc(tfb200_mask_attn_bwd_f32(q.data_ptr<float>(), k.data_ptr<float>(), w.data_ptr<float>(), dwc.data_ptr<float>(),
+                                    ds.data_ptr<float>(), dq.data_ptr<float>(), dk.data_ptr<float>(), B, Q, HW, heads,
+                                    float(scale), c10::cuda::getCurrentCUDAStream().stream()),
+           "mask_attn_backward");
+  return {dq, dk};
+}
+
+static const float* opt_addend(const c10::optional<at::Tensor>& addend, const at::Tensor& x, int per_image) {
+  if (!addend.has_value() || !addend->defined()) return nullptr;
+  check_nhwc(*addend, "group_norm_relu addend");
+  TORCH_CHECK(addend->size(0) * per_image == x.size(0) && addend->size(1) == x.size(1) && addend->size(2) == x.size(2) &&
+              addend->size(3) == x.size(3), "group_norm_relu: addend must be [N / per_image, C, H, W]");
+  return addend->data_ptr<float>();
+}
+
+// x [N, C, H, W] channels-last (+ addend [N / per_image, C, H, W]) -> {y, mean [N, G], rstd [N, G]}
+std::vector<at::Tensor> group_norm_relu_forward(const at::Tensor& x, const c10::optional<at::Tensor>& addend,
+                                                const at::Tensor& gamma, const at::Tensor& beta, int64_t groups,
+                                                int64_t per_image, double eps) {
+  check_nhwc(x, "group_norm_relu x");
+  TORCH_CHECK(per_image > 0 && x.size(0) % per_image == 0, "group_norm_relu: N must be a multiple of per_image");
+  const int64_t C = x.size(1);
+  check_f32(gamma, "group_norm_relu gamma");
+  check_f32(beta, "group_norm_relu beta");
+  TORCH_CHECK(gamma.numel() == C && beta.numel() == C && gamma.is_contiguous() && beta.is_contiguous(),
+              "group_norm_relu: gamma / beta [C]");
+  const float* ap = opt_addend(addend, x, int(per_image));
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor y = empty_nhwc(x.sizes(), x);
+  at::Tensor mean = at::empty({x.size(0), groups}, x.options()), rstd = at::empty({x.size(0), groups}, x.options());
+  raise_rc(tfb200_group_norm_relu_fwd_f32(x.data_ptr<float>(), ap, gamma.data_ptr<float>(), beta.data_ptr<float>(),
+                                          y.data_ptr<float>(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
+                                          int(x.size(0)), int(per_image), x.size(2) * x.size(3), int(C), int(groups),
+                                          float(eps), c10::cuda::getCurrentCUDAStream().stream()),
+           "group_norm_relu_forward");
+  return {y, mean, rstd};
+}
+
+// -> {dx, daddend (undefined without addend), dgamma, dbeta}
+std::vector<at::Tensor> group_norm_relu_backward(const at::Tensor& dy, const at::Tensor& x,
+                                                 const c10::optional<at::Tensor>& addend, const at::Tensor& y,
+                                                 const at::Tensor& gamma, const at::Tensor& mean, const at::Tensor& rstd,
+                                                 int64_t per_image) {
+  check_nhwc(x, "group_norm_relu x");
+  check_nhwc(y, "group_norm_relu y");
+  check_f32(dy, "group_norm_relu dy");
+  TORCH_CHECK(dy.sizes() == x.sizes() && y.sizes() == x.sizes() && per_image > 0 && x.size(0) % per_image == 0,
+              "group_norm_relu_backward: dy, x, y must have one shape");
+  const at::Tensor dyc = dy.contiguous(at::MemoryFormat::ChannelsLast);
+  const int64_t N = x.size(0), C = x.size(1);
+  const float* ap = opt_addend(addend, x, int(per_image));
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor dx = empty_nhwc(x.sizes(), x);
+  at::Tensor da = ap ? empty_nhwc(addend->sizes(), x) : at::Tensor();
+  at::Tensor daff = at::empty({2, C}, x.options()), ws = at::empty({N, 2, C}, x.options());
+  raise_rc(tfb200_group_norm_relu_bwd_f32(dyc.data_ptr<float>(), x.data_ptr<float>(), ap, y.data_ptr<float>(),
+                                          gamma.data_ptr<float>(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
+                                          dx.data_ptr<float>(), ap ? da.data_ptr<float>() : nullptr, daff.data_ptr<float>(),
+                                          ws.data_ptr<float>(), int(N), int(per_image), x.size(2) * x.size(3), int(C),
+                                          int(mean.size(1)), c10::cuda::getCurrentCUDAStream().stream()),
+           "group_norm_relu_backward");
+  return {dx, da, daff[0], daff[1]};
+}
+
+// a [N / per_image, C, Ho, Wo] + nearest_upsample(x [N, C, Hi, Wi]), both channels-last
+at::Tensor upsample_add_forward(const at::Tensor& x, const at::Tensor& a) {
+  check_nhwc(x, "upsample_add x");
+  check_nhwc(a, "upsample_add a");
+  TORCH_CHECK(a.size(0) > 0 && x.size(0) % a.size(0) == 0 && a.size(1) == x.size(1),
+              "upsample_add: x [N, C, Hi, Wi] and a [N / per_image, C, Ho, Wo]");
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor out = empty_nhwc({x.size(0), x.size(1), a.size(2), a.size(3)}, x);
+  raise_rc(tfb200_upsample_add_fwd_f32(x.data_ptr<float>(), a.data_ptr<float>(), out.data_ptr<float>(), int(x.size(0)),
+                                       int(x.size(0) / a.size(0)), int(x.size(2)), int(x.size(3)), int(a.size(2)),
+                                       int(a.size(3)), int(x.size(1)), c10::cuda::getCurrentCUDAStream().stream()),
+           "upsample_add_forward");
+  return out;
+}
+
+std::vector<at::Tensor> upsample_add_backward(const at::Tensor& dout, int64_t images, int64_t Hi, int64_t Wi) {
+  check_f32(dout, "upsample_add dout");
+  TORCH_CHECK(dout.dim() == 4 && images > 0 && dout.size(0) % images == 0 && Hi > 0 && Wi > 0,
+              "upsample_add_backward: dout [N, C, Ho, Wo]");
+  const at::Tensor g = dout.contiguous(at::MemoryFormat::ChannelsLast);
+  const int64_t N = g.size(0), C = g.size(1);
+  const c10::cuda::CUDAGuard guard(g.device());
+  at::Tensor dx = empty_nhwc({N, C, Hi, Wi}, g), da = empty_nhwc({images, C, g.size(2), g.size(3)}, g);
+  raise_rc(tfb200_upsample_add_bwd_f32(g.data_ptr<float>(), dx.data_ptr<float>(), da.data_ptr<float>(), int(N),
+                                       int(N / images), int(Hi), int(Wi), int(g.size(2)), int(g.size(3)), int(C),
+                                       c10::cuda::getCurrentCUDAStream().stream()),
+           "upsample_add_backward");
+  return {dx, da};
+}
+
+static void check_mask_loss_args(const at::Tensor& logits, const at::Tensor& src, const at::Tensor& tgt_masks,
+                                 const at::Tensor& tgt, const at::Tensor& num_boxes) {
+  check_f32(logits, "mask_loss logits");
+  TORCH_CHECK(logits.dim() == 3 && logits.is_contiguous(), "mask_loss: logits must be a contiguous [R, h, w] tensor");
+  TORCH_CHECK(tgt_masks.is_cuda() && tgt_masks.dim() == 3 && tgt_masks.element_size() == 1 &&
+              tgt_masks.scalar_type() != at::kChar && tgt_masks.is_contiguous(),
+              "mask_loss: target masks must be a contiguous bool/uint8 [T, Ht, Wt] CUDA tensor");
+  TORCH_CHECK(src.is_cuda() && tgt.is_cuda() && src.scalar_type() == at::kLong && tgt.scalar_type() == at::kLong &&
+              src.dim() == 1 && src.sizes() == tgt.sizes() && src.is_contiguous() && tgt.is_contiguous(),
+              "mask_loss: src / tgt must be int64 [M] CUDA tensors");
+  check_f32(num_boxes, "mask_loss num_boxes");
+  TORCH_CHECK(num_boxes.numel() == 1, "mask_loss: num_boxes must be a one-element tensor");
+}
+
+// -> {out [2] = (loss_mask, loss_dice), stats [M, 4]}
+std::vector<at::Tensor> mask_loss_forward(const at::Tensor& logits, const at::Tensor& src, const at::Tensor& tgt_masks,
+                                          const at::Tensor& tgt, const at::Tensor& num_boxes, double alpha, double gamma) {
+  check_mask_loss_args(logits, src, tgt_masks, tgt, num_boxes);
+  const int M = int(src.numel()), Ht = int(tgt_masks.size(1)), Wt = int(tgt_masks.size(2));
+  const c10::cuda::CUDAGuard guard(logits.device());
+  at::Tensor out = at::empty({2}, logits.options()), stats = at::empty({M, 4}, logits.options());
+  at::Tensor ws = at::empty({M, tfb200_mask_loss_partial_chunks(Ht, Wt), 4}, logits.options());
+  raise_rc(tfb200_mask_loss_fwd_f32(logits.data_ptr<float>(), src.data_ptr<int64_t>(),
+                                    reinterpret_cast<const uint8_t*>(tgt_masks.data_ptr()), tgt.data_ptr<int64_t>(),
+                                    num_boxes.data_ptr<float>(), stats.data_ptr<float>(), ws.data_ptr<float>(),
+                                    out.data_ptr<float>(), M, int(logits.size(1)), int(logits.size(2)), Ht, Wt,
+                                    float(alpha), float(gamma), c10::cuda::getCurrentCUDAStream().stream()),
+           "mask_loss_forward");
+  return {out, stats};
+}
+
+at::Tensor mask_loss_backward(const at::Tensor& logits, const at::Tensor& src, const at::Tensor& tgt_masks,
+                              const at::Tensor& tgt, const at::Tensor& stats, const at::Tensor& num_boxes,
+                              const at::Tensor& g2, double alpha, double gamma) {
+  check_mask_loss_args(logits, src, tgt_masks, tgt, num_boxes);
+  check_f32(g2, "mask_loss g2");
+  TORCH_CHECK(g2.numel() == 2 && stats.numel() == src.numel() * 4, "mask_loss_backward: g2 [2], stats [M, 4]");
+  const at::Tensor gc = g2.contiguous();
+  const c10::cuda::CUDAGuard guard(logits.device());
+  at::Tensor grad = at::empty_like(logits);
+  raise_rc(tfb200_mask_loss_bwd_f32(logits.data_ptr<float>(), src.data_ptr<int64_t>(),
+                                    reinterpret_cast<const uint8_t*>(tgt_masks.data_ptr()), tgt.data_ptr<int64_t>(),
+                                    stats.data_ptr<float>(), num_boxes.data_ptr<float>(), gc.data_ptr<float>(),
+                                    grad.data_ptr<float>(), int(logits.size(0)), int(src.numel()), int(logits.size(1)),
+                                    int(logits.size(2)), int(tgt_masks.size(1)), int(tgt_masks.size(2)), float(alpha),
+                                    float(gamma), c10::cuda::getCurrentCUDAStream().stream()),
+           "mask_loss_backward");
+  return grad;
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100 (sm_90a) multi-scale deformable attention; drop-in for the reference extension";
   m.def("ms_deform_attn_forward", &ms_deform_attn_forward, "ms_deform_attn_forward");
@@ -821,4 +1017,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("frozen_bn_act_forward", &frozen_bn_act_forward);
   m.def("frozen_bn_act_backward", &frozen_bn_act_backward);
   m.def("frozen_bn_relu_maxpool", &frozen_bn_relu_maxpool);
+  m.def("mask_attn_forward", &mask_attn_forward);
+  m.def("mask_attn_backward", &mask_attn_backward);
+  m.def("group_norm_relu_forward", &group_norm_relu_forward);
+  m.def("group_norm_relu_backward", &group_norm_relu_backward);
+  m.def("upsample_add_forward", &upsample_add_forward);
+  m.def("upsample_add_backward", &upsample_add_backward);
+  m.def("mask_loss_forward", &mask_loss_forward);
+  m.def("mask_loss_backward", &mask_loss_backward);
 }

@@ -4,6 +4,10 @@
 configurations (detection and tracking): it returns ``(model, criterion, postprocessors)`` with the same class
 counts (:17-26), loss weights (:83-99) and focal-loss post-processor (:117-118).
 
+With ``masks=True`` it builds the segmentation models of src/trackformer/models/detr_segmentation.py
+(``DeformableDETRSegm`` / ``DeformableDETRSegmTracking``) and adds the ``masks`` loss and the ``segm``
+post-processor (:42-45, 86-88, 103-104, 121-125); the panoptic post-processor is not provided.
+
 ``default_args(...)`` reproduces the values of cfgs/train.yaml overlaid with train_deformable.yaml and,
 optionally, train_tracking.yaml / train_multi_frame.yaml (the named sacred configs of src/train.py:24-35), so
 the benchmark and the tests can instantiate the exact reference geometry without the YAML files (they do not
@@ -21,6 +25,7 @@ from .deformable_detr import DeformableDETR, DeformablePostProcess
 from .deformable_transformer import build_deforamble_transformer
 from .detr_tracking import DeformableDETRTracking
 from .matcher import build_matcher
+from .segmentation import DeformableDETRSegm, DeformableDETRSegmTracking, PostProcessSegm
 
 _TRAIN_YAML = dict(   # cfgs/train.yaml (model / loss keys only)
     lr=2e-4, lr_backbone_names=["backbone.0"], lr_backbone=2e-5,
@@ -75,8 +80,8 @@ def num_classes_for(dataset: str) -> int:
 def build_model(args):
     if not args.deformable:
         raise NotImplementedError("only the deformable path is built (vanilla DETR is outside the hot path)")
-    if args.masks:
-        raise NotImplementedError("segmentation heads are outside the hot path")
+    if args.masks and args.dataset == "coco_panoptic":
+        raise NotImplementedError("the panoptic post-processor is not provided")
     num_classes = num_classes_for(args.dataset)
     backbone = build_backbone(args)
     matcher = build_matcher(args)
@@ -92,20 +97,30 @@ def build_model(args):
             track_query_false_positive_prob=args.track_query_false_positive_prob,
             track_query_false_negative_prob=args.track_query_false_negative_prob,
             matcher=matcher, backprop_prev_frame=args.track_backprop_prev_frame)
-        model = DeformableDETRTracking(tracking_kwargs, detr_kwargs)
+        if args.masks:
+            model = DeformableDETRSegmTracking({"freeze_detr": args.freeze_detr}, tracking_kwargs, detr_kwargs)
+        else:
+            model = DeformableDETRTracking(tracking_kwargs, detr_kwargs)
+    elif args.masks:
+        model = DeformableDETRSegm({"freeze_detr": args.freeze_detr}, detr_kwargs)
     else:
         model = DeformableDETR(**detr_kwargs)
 
     weight_dict = {"loss_ce": args.cls_loss_coef, "loss_bbox": args.bbox_loss_coef, "loss_giou": args.giou_loss_coef}
+    if args.masks:
+        weight_dict["loss_mask"] = args.mask_loss_coef
+        weight_dict["loss_dice"] = args.dice_loss_coef
     if args.aux_loss:
         base = dict(weight_dict)
         for i in range(args.dec_layers - 1):
             weight_dict.update({f"{k}_{i}": v for k, v in base.items()})
     criterion = SetCriterion(
         num_classes, matcher=matcher, weight_dict=weight_dict, eos_coef=args.eos_coef,
-        losses=["labels", "boxes", "cardinality"], focal_loss=args.focal_loss, focal_alpha=args.focal_alpha,
+        losses=["labels", "boxes", "cardinality"] + (["masks"] if args.masks else []), focal_loss=args.focal_loss, focal_alpha=args.focal_alpha,
         focal_gamma=args.focal_gamma, tracking=args.tracking,
         track_query_false_positive_eos_weight=args.track_query_false_positive_eos_weight)
     criterion.to(torch.device(args.device))
     postprocessors = {"bbox": DeformablePostProcess()}
+    if args.masks:
+        postprocessors["segm"] = PostProcessSegm()
     return model, criterion, postprocessors

@@ -56,6 +56,9 @@ class TrainStep:
         """``optimizer_factory(params)`` builds any torch optimizer; ``flat_adamw={'groups': [...], 'betas':..., 'eps':...}``
         (groups as for torch.optim.AdamW, e.g. flat_adamw.reference_param_groups(model)) instead lays the PARAMETERS out
         flat as well and updates them with the one-pass clip + AdamW kernel."""
+        if hasattr(model, "mask_head") or "masks" in getattr(criterion, "losses", ()):
+            raise NotImplementedError("TrainStep does not train segmentation models (their mask losses would be "
+                                      "dropped); run the model and SetCriterion eagerly instead")
         self.model = model
         self.criterion = criterion
         self.max_norm = max_norm

@@ -165,6 +165,14 @@ def sigmoid_focal_loss(logits: Tensor, targets: Tensor, num_boxes: float, alpha:
     return loss.mean(1).sum() / num_boxes
 
 
+def dice_loss(logits: Tensor, targets: Tensor, num_boxes: float) -> Tensor:
+    """DICE loss of sigmoid(logits) against binary targets, per row, summed and divided by num_boxes (util/misc.py:522-537)."""
+    p = logits.sigmoid().flatten(1)
+    numerator = 2 * (p * targets).sum(1)
+    denominator = p.sum(-1) + targets.sum(-1)
+    return (1 - (numerator + 1) / (denominator + 1)).sum() / num_boxes
+
+
 @torch.no_grad()
 def accuracy(output: Tensor, target: Tensor, topk=(1,)) -> List[Tensor]:
     if target.numel() == 0:
