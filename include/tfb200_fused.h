@@ -184,7 +184,8 @@ int tfb200_small_attn_bwd_f32(const float* q, const float* k, const float* v, co
  * tracks are used for this frame's object queries: capacity >= n_active + n_inactive + nq, <= 2048); `out` receives
  * the new state, `q_boxes` / `q_embeds` the track queries of the next frame (active tracks, then the inactive ones that
  * survive the patience / positive-area test, boxes as cx, cy, w, h divided by the image size), and `result` the header
- * followed by n_results rows of 8 words {id, obj_ind, score, x0, y0, x1, y1, 0} (ints and fp32 bit patterns).
+ * followed by n_results rows of 8 words {id, obj_ind, score, x0, y0, x1, y1, src} (ints and fp32 bit patterns); src is
+ * the query row whose embedding -- and so whose segmentation mask -- the track took this frame, or -1 if it took none.
  * error: 1 = n_query does not match the state, 2 = capacity.                                                         */
 typedef struct TfbTrackState {
   int32_t* header;             /* [8] */
@@ -260,6 +261,18 @@ int tfb200_mask_loss_fwd_f32(const float* logits, const int64_t* src, const uint
 int tfb200_mask_loss_bwd_f32(const float* logits, const int64_t* src, const uint8_t* tgt_masks, const int64_t* tgt,
                              const float* stats, const float* num_boxes, const float* g2, float* grad_logits, int R,
                              int M, int h, int w, int Ht, int Wt, float alpha, float gamma, void* stream);
+
+/* Segmentation masks of the tracker's active tracks resolved into one label map (csrc/track_masks.cu; reference
+ * models/detr_segmentation.py:219-253 with return_probs=True, models/tracker.py:509-521).  T tracks in active-list
+ * order; src[t] is the row of logits [K][h][w] (stride-4 mask logits) the track takes this frame, or -1 for a track
+ * that keeps its previous mask, which is prev_label == ids[t] (value exactly 1.0).  A fresh track's value at output
+ * pixel (y, x) of [H][W] is sigmoid(bilinear (align_corners=False) upsampling to [size_h][size_w]) at the nearest
+ * source pixel of the [crop_h][crop_w] crop.  label[y][x] = ids[first t of maximal value] if that value > 0.5, else
+ * -1.  ids >= 0 and unique; logits may be NULL when no src is >= 0; prev_label [H][W] or NULL (no stale tracks).
+ * T == 0 writes nothing.                                                                                          */
+int tfb200_track_masks_f32(const float* logits, const int32_t* src, const int32_t* ids, const int32_t* prev_label,
+                           int32_t* label, int T, int h, int w, int size_h, int size_w, int crop_h, int crop_w, int H,
+                           int W, void* stream);
 
 #ifdef __cplusplus
 }

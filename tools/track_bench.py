@@ -7,6 +7,12 @@ timed step is the whole `Tracker.step(blob)`: host frame -> device, forward, fus
 bookkeeping.  Random weights give flat scores, so the live-track count is pinned by thresholds: the first frame starts
 exactly `--tracks` tracks, afterwards every track is kept and no new ones start.
 
+`--masks` tracks with the segmentation model (DeformableDETRSegmTracking, "segm" post-processing): Tracker and
+DeviceTracker over the CUDA-graph detector, each running the mask head on the rows the frame's decisions keep and
+resolving the masks into one label map, against the reference-shaped work for the same frame -- the full forward with
+`pred_masks` for every query row plus PostProcessSegm(return_probs=True), which upsamples every row to the image and
+copies it to the host.
+
 Prints one JSON line; tools/README.md lists it among the measurement aids.  Not a bench.py arm.
 """
 import argparse
@@ -33,6 +39,7 @@ def main():
     ap.add_argument("--bucket", type=int, default=32)
     ap.add_argument("--no-tf32", action="store_true")
     ap.add_argument("--skip-eager", action="store_true", help="only the CUDA-graph detector")
+    ap.add_argument("--masks", action="store_true", help="segmentation model, tracking with masks")
     args = ap.parse_args()
     from trackformer_b200.deformable_detr import DeformablePostProcess
     from trackformer_b200.graphed_detector import GraphedDetector
@@ -43,7 +50,7 @@ def main():
     dev = torch.device("cuda:0")
     torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = not args.no_tf32
     torch.manual_seed(0)
-    model, _, _ = build_model(default_args(True, args.multi_frame, device="cuda:0"))
+    model, _, _ = build_model(default_args(True, args.multi_frame, device="cuda:0", **({"masks": True} if args.masks else {})))
     with torch.no_grad():
         for name, p in model.named_parameters():               # make class 0 the winning label (random weights)
             if "class_embed" in name and name.endswith("bias"):
@@ -58,9 +65,19 @@ def main():
                reid_greedy_matching=False)
     size = torch.tensor([[args.height, args.width]])
 
+    def blob(i):
+        b = {"img": frames[i % 4], "orig_size": size, "dets": torch.zeros(1, 0, 4)}
+        if args.masks:
+            b["size"] = size
+        return b
+
     def run(detector, tracker_cls=Tracker):
         post = DeformablePostProcess()
-        tr = tracker_cls(detector, {"bbox": post}, cfg, False)
+        posts = {"bbox": post}
+        if args.masks:
+            from trackformer_b200.segmentation import PostProcessSegm
+            posts["segm"] = PostProcessSegm()
+        tr = tracker_cls(detector, posts, cfg, False)
         tr.reset()
         # frame 0: start exactly --tracks tracks
         with torch.no_grad():
@@ -69,20 +86,26 @@ def main():
         s = np.sort(rows[rows[:, 1] == 0, 0])[::-1]
         assert len(s) > args.tracks, "not enough class-0 queries to start the requested number of tracks"
         tr.detection_obj_score_thresh = float((s[args.tracks - 1] + s[args.tracks]) / 2)
-        tr.step({"img": frames[0], "orig_size": size, "dets": torch.zeros(1, 0, 4)})
+        tr.step(blob(0))
         tr.detection_obj_score_thresh = 2.0
         assert len(tr.tracks) == args.tracks, len(tr.tracks)
         times = []
         for i in range(args.warmup + args.frames):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
-            tr.step({"img": frames[(i + 1) % 4], "orig_size": size, "dets": torch.zeros(1, 0, 4)})
+            tr.step(blob(i + 1))
             torch.cuda.synchronize()
             if i >= args.warmup:
                 times.append((time.perf_counter() - t0) * 1e3)
         assert len(tr.tracks) == args.tracks
+        if args.masks:
+            head_rows.append(int((tr._result_rows >= 0).sum()))
         return times
 
+    head_rows = []
+    if args.masks:
+        print(json.dumps(masks_line(args, model, frames, size, dev, run, head_rows)))
+        return
     det = GraphedDetector(model, bucket=args.bucket)
     graphed = run(det)
     eager = graphed if args.skip_eager else run(model)
@@ -103,6 +126,50 @@ def main():
         "d2h_bytes_per_frame_device_tracker": int((8 + 8 * (args.tracks + model.num_queries)) * 4),
     }
     print(json.dumps(line))
+
+
+def masks_line(args, model, frames, size, dev, run, head_rows):
+    from trackformer_b200.device_tracker import DeviceTracker
+    from trackformer_b200.graphed_detector import GraphedDetector
+    from trackformer_b200.segmentation import PostProcessSegm
+
+    # the reference-shaped work of one frame: full forward (pred_masks for all rows) + PostProcessSegm to the host
+    post = PostProcessSegm()
+    with torch.no_grad():
+        out, _, feats, _, _ = model(frames[0].to(dev), None, None)
+        tgt = [{"track_query_boxes": out["pred_boxes"][0, :args.tracks].clone(),
+                "track_query_hs_embeds": out["hs_embed"][0, :args.tracks].clone(),
+                "image_id": torch.tensor([1], device=dev)}]
+        full = []
+        for i in range(args.warmup + args.frames):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            o, _, feats, _, _ = model(frames[(i + 1) % 4].to(dev), tgt, feats)
+            post([{}], o, size.to(dev), size.to(dev), return_probs=True)
+            torch.cuda.synchronize()
+            if i >= args.warmup:
+                full.append((time.perf_counter() - t0) * 1e3)
+        n_rows = args.tracks + model.num_queries
+        del out, o
+    torch.cuda.empty_cache()
+    host = run(GraphedDetector(model, bucket=args.bucket))
+    device = run(GraphedDetector(model, bucket=args.bucket), DeviceTracker)
+
+    def stats(t):
+        return {"median": float(np.median(t)), "p10": float(np.percentile(t, 10)), "p90": float(np.percentile(t, 90))}
+    label_bytes = args.height * args.width * 4
+    return {
+        "what": "Tracker.step latency with segmentation masks, host frame in -> results (with masks) out",
+        "frames": args.frames, "warmup": args.warmup,
+        "config": {"workload": f"segmentation tracking 1x3x{args.height}x{args.width}, {args.tracks} track + "
+                               f"{model.num_queries} object queries", "bucket": args.bucket, "tf32": not args.no_tf32},
+        "graph_masks_ms": stats(host), "graph_device_tracker_masks_ms": stats(device),
+        "reference_shaped_forward_plus_postprocess_segm_ms": stats(full),
+        "head_rows_per_frame": head_rows, "head_rows_per_frame_reference_shaped": n_rows,
+        "d2h_bytes_per_frame": int(n_rows * 6 * 4 + label_bytes),
+        "d2h_bytes_per_frame_device_tracker": int((8 + 8 * n_rows) * 4 + label_bytes),
+        "d2h_bytes_per_frame_reference_shaped": int(n_rows * args.height * args.width * 4),
+    }
 
 
 if __name__ == "__main__":

@@ -975,6 +975,40 @@ at::Tensor mask_loss_backward(const at::Tensor& logits, const at::Tensor& src, c
   return grad;
 }
 
+// ---- tracker segmentation masks (csrc/track_masks.cu) ----
+// logits [K, h, w] fp32, src / ids [T] int32, prev_label [H, W] int32 or None -> label [H, W] int32
+at::Tensor track_masks(const at::Tensor& logits, const at::Tensor& src, const at::Tensor& ids,
+                       const c10::optional<at::Tensor>& prev_label, int64_t size_h, int64_t size_w, int64_t crop_h,
+                       int64_t crop_w, int64_t H, int64_t W) {
+  check_f32(logits, "track_masks logits");
+  TORCH_CHECK(logits.dim() == 3, "track_masks: logits must be [K, h, w]");
+  auto check_i32 = [&](const at::Tensor& t, const char* what) {
+    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kInt && t.device() == logits.device(), what,
+                ": int32 CUDA tensor on the logits' device required");
+  };
+  check_i32(src, "track_masks src");
+  check_i32(ids, "track_masks ids");
+  TORCH_CHECK(src.dim() == 1 && src.sizes() == ids.sizes(), "track_masks: src and ids must be [T]");
+  const at::Tensor lc = logits.contiguous(), sc = src.contiguous(), ic = ids.contiguous();
+  at::Tensor pc;
+  if (prev_label.has_value() && prev_label->defined()) {
+    check_i32(*prev_label, "track_masks prev_label");
+    TORCH_CHECK(prev_label->dim() == 2 && prev_label->size(0) == H && prev_label->size(1) == W,
+                "track_masks: prev_label must be [H, W]");
+    pc = prev_label->contiguous();
+  }
+  const c10::cuda::CUDAGuard guard(logits.device());
+  at::Tensor label = at::full({H, W}, -1, ids.options());
+  if (src.numel() == 0) return label;                  // no active track: all background (empty tensors have no data)
+  raise_rc(tfb200_track_masks_f32(lc.numel() ? lc.data_ptr<float>() : nullptr, sc.data_ptr<int32_t>(),
+                                  ic.data_ptr<int32_t>(), pc.defined() ? pc.data_ptr<int32_t>() : nullptr,
+                                  label.data_ptr<int32_t>(), int(src.numel()), int(logits.size(1)),
+                                  int(logits.size(2)), int(size_h), int(size_w), int(crop_h), int(crop_w), int(H),
+                                  int(W), c10::cuda::getCurrentCUDAStream().stream()),
+           "track_masks");
+  return label;
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100 (sm_90a) multi-scale deformable attention; drop-in for the reference extension";
   m.def("ms_deform_attn_forward", &ms_deform_attn_forward, "ms_deform_attn_forward");
@@ -1025,4 +1059,5 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("upsample_add_backward", &upsample_add_backward);
   m.def("mask_loss_forward", &mask_loss_forward);
   m.def("mask_loss_backward", &mask_loss_backward);
+  m.def("track_masks", &track_masks);
 }

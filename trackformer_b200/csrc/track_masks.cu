@@ -1,0 +1,208 @@
+// Segmentation masks of the online tracker's active tracks, resolved in one launch (sm_90a).
+//
+// Reference: src/trackformer/models/detr_segmentation.py:219-253 (PostProcessSegm with return_probs=True) followed by
+// src/trackformer/models/tracker.py:509-521.  The reference upsamples the stride-4 mask logits of EVERY query row
+// bilinearly to the padded input size, applies the sigmoid, copies all of it to the host, crops each row to the image
+// and nearest-resizes it to the original size; at the end of the frame the active tracks' masks are stacked (a track
+// that did not take a new mask keeps the boolean mask of the previous frame, promoted to 0 / 1 by torch.stack) and every
+// pixel goes to the FIRST track of maximal value when that value exceeds 0.5.
+//
+// Here the same value is computed per output pixel, for the active tracks only, and the resolved masks leave the device
+// as one int32 label map (track id, or -1 for background):
+//   * the nearest and bilinear source indices / weights of a pixel are computed once and serve every track;
+//   * the low-resolution footprint of an output tile is staged in shared memory for a chunk of tracks at a time, so the
+//     number of tracks is unbounded (a footprint larger than the stage reads global memory instead);
+//   * the running (best value, first position) pair of each pixel stays in registers; a strict '>' in list order keeps
+//     the first maximum, so exact ties (saturated sigmoids, stale masks at exactly 1.0) resolve like torch.argmax;
+//   * stale tracks cost one read of the previous label map per pixel and one lookup in a shared-memory hash table
+//     (id -> list position), never a scan over the stale tracks.
+// Index maths is ATen's (UpSample.h): nearest_idx with its identity and 2x cases and fp32 scale, and
+// area_pixel_compute_source_index (align_corners=False) with the clamp at 0 and the "+1 if < size - 1" neighbour.  The
+// interpolation and the sigmoid are evaluated in fp32 without contraction, in the order of ATen's CPU kernel.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+
+#include "../../include/tfb200_fused.h"
+#include "launch_counter.h"
+
+namespace {
+
+constexpr int kTileW = 64;                 // output tile: 64 columns x 16 rows, 256 threads, 4 rows per thread
+constexpr int kTileH = 16;
+constexpr int kThreads = 256;
+constexpr int kRows = kTileH / (kThreads / kTileW);
+constexpr int kMaxChunk = 256;             // tracks per pass over the output tile
+constexpr int kStageFloats = 8192;         // 32 KB of staged logits per pass
+constexpr int kMaxSmem = 200 * 1024;
+
+struct Lin {
+  int i0, i1;
+  float l0, l1;
+};
+
+// ATen nearest_idx (UpSample.h) for input size `in`, output size `out`
+__device__ __forceinline__ int nearest_src(int o, int in, int out) {
+  if (out == in) return o;
+  if (out == 2 * in) return o >> 1;
+  const float scale = float(in) / float(out);
+  return min(int(floorf(__fmul_rn(float(o), scale))), in - 1);
+}
+
+// ATen compute_source_index_and_lambda, linear mode, align_corners=False
+__device__ __forceinline__ Lin linear_src(int o, int in, int out) {
+  if (out == in) return {o, o, 1.f, 0.f};
+  const float scale = float(in) / float(out);
+  float s = __fsub_rn(__fmul_rn(scale, __fadd_rn(float(o), 0.5f)), 0.5f);
+  s = s < 0.f ? 0.f : s;
+  const int i0 = min(int(floorf(s)), in - 1);
+  const float l1 = fminf(fmaxf(__fsub_rn(s, float(i0)), 0.f), 1.f);
+  return {i0, i0 + (i0 < in - 1 ? 1 : 0), __fsub_rn(1.f, l1), l1};
+}
+
+__device__ __forceinline__ unsigned slot_of(int id, int mask) {
+  unsigned x = unsigned(id);
+  x = (x ^ (x >> 16)) * 0x45d9f3bu;
+  x = (x ^ (x >> 16)) * 0x45d9f3bu;
+  return (x ^ (x >> 16)) & unsigned(mask);
+}
+
+__global__ void __launch_bounds__(kThreads, 2)
+track_masks_kernel(const float* __restrict__ logits, const int32_t* __restrict__ src, const int32_t* __restrict__ ids,
+                   const int32_t* __restrict__ prev, int32_t* __restrict__ label, int T, int h, int w, int size_h,
+                   int size_w, int crop_h, int crop_w, int H, int W, int hash_slots) {
+  extern __shared__ int smem[];
+  int* hkey = smem;
+  int* hval = hkey + hash_slots;
+  int* csrc = hval + hash_slots;
+  float* stage = reinterpret_cast<float*>(csrc + kMaxChunk);
+  const int tid = threadIdx.x, tx = tid % kTileW, ty = tid / kTileW;
+
+  // ---- stale tracks: id -> list position
+  if (prev != nullptr) {
+    for (int i = tid; i < hash_slots; i += kThreads) hkey[i] = -1;
+    __syncthreads();
+    for (int t = tid; t < T; t += kThreads) {
+      if (src[t] >= 0) continue;
+      const int id = ids[t];
+      unsigned s = slot_of(id, hash_slots - 1);
+      while (true) {
+        const int old = atomicCAS(hkey + s, -1, id);
+        if (old == -1 || old == id) { hval[s] = t; break; }
+        s = (s + 1) & unsigned(hash_slots - 1);
+      }
+    }
+  }
+
+  // ---- source indices of this thread's pixels, and the tile's low-resolution footprint (indices are monotone)
+  const int x0_tile = blockIdx.x * kTileW, y0_tile = blockIdx.y * kTileH;
+  const int x_last = min(x0_tile + kTileW, W) - 1, y_last = min(y0_tile + kTileH, H) - 1;
+  const int fx0 = linear_src(nearest_src(x0_tile, crop_w, W), w, size_w).i0;
+  const int fx1 = linear_src(nearest_src(x_last, crop_w, W), w, size_w).i1;
+  const int fy0 = linear_src(nearest_src(y0_tile, crop_h, H), h, size_h).i0;
+  const int fy1 = linear_src(nearest_src(y_last, crop_h, H), h, size_h).i1;
+  const int fw = fx1 - fx0 + 1, fp = (fy1 - fy0 + 1) * fw;
+  const bool staged = fp <= kStageFloats;
+  const int chunk = staged ? min(kMaxChunk, kStageFloats / fp) : kMaxChunk;
+  const int row_stride = staged ? fw : w;
+
+  const int x = x0_tile + tx;
+  const Lin lx = linear_src(nearest_src(min(x, W - 1), crop_w, W), w, size_w);
+  const int c0 = staged ? lx.i0 - fx0 : lx.i0, c1 = staged ? lx.i1 - fx0 : lx.i1;
+  int r0[kRows], r1[kRows];
+  float h0[kRows], h1[kRows], best[kRows];
+  int pos[kRows];
+#pragma unroll
+  for (int r = 0; r < kRows; ++r) {
+    const int y = min(y0_tile + ty + r * (kThreads / kTileW), H - 1);
+    const Lin ly = linear_src(nearest_src(y, crop_h, H), h, size_h);
+    r0[r] = (staged ? ly.i0 - fy0 : ly.i0) * row_stride;
+    r1[r] = (staged ? ly.i1 - fy0 : ly.i1) * row_stride;
+    h0[r] = ly.l0;
+    h1[r] = ly.l1;
+    best[r] = -1.f;                        // below every probability
+    pos[r] = -1;
+  }
+
+  // ---- fresh tracks, in list order, a chunk at a time
+  const int64_t plane = int64_t(h) * w;
+  for (int t0 = 0; t0 < T; t0 += chunk) {
+    const int n = min(chunk, T - t0);
+    __syncthreads();                       // previous chunk fully consumed (and the hash table built)
+    for (int i = tid; i < n; i += kThreads) csrc[i] = src[t0 + i];
+    __syncthreads();
+    if (staged) {
+      for (int e = tid; e < n * fp; e += kThreads) {
+        const int k = e / fp, q = e - k * fp;
+        const int s = csrc[k];
+        if (s >= 0) stage[e] = __ldg(logits + s * plane + int64_t(fy0 + q / fw) * w + fx0 + q % fw);
+      }
+      __syncthreads();
+    }
+    for (int k = 0; k < n; ++k) {
+      const int s = csrc[k];
+      if (s < 0) continue;
+      const float* base = staged ? stage + k * fp : logits + s * plane;
+#pragma unroll
+      for (int r = 0; r < kRows; ++r) {
+        const float a = __fadd_rn(__fmul_rn(base[r0[r] + c0], lx.l0), __fmul_rn(base[r0[r] + c1], lx.l1));
+        const float b = __fadd_rn(__fmul_rn(base[r1[r] + c0], lx.l0), __fmul_rn(base[r1[r] + c1], lx.l1));
+        const float v = __fadd_rn(__fmul_rn(a, h0[r]), __fmul_rn(b, h1[r]));
+        const float p = 1.f / (1.f + expf(-v));
+        if (p > best[r]) { best[r] = p; pos[r] = t0 + k; }
+      }
+    }
+  }
+  // (T > 0, so the first pass's barrier has also published the hash table)
+
+  // ---- stale candidate (value exactly 1.0), threshold, label
+  if (x >= W) return;
+#pragma unroll
+  for (int r = 0; r < kRows; ++r) {
+    const int y = y0_tile + ty + r * (kThreads / kTileW);
+    if (y >= H) continue;
+    const int64_t o = int64_t(y) * W + x;
+    if (prev != nullptr) {
+      const int id = prev[o];
+      if (id >= 0) {
+        unsigned s = slot_of(id, hash_slots - 1);
+        while (hkey[s] != -1 && hkey[s] != id) s = (s + 1) & unsigned(hash_slots - 1);
+        if (hkey[s] == id) {
+          const int t = hval[s];
+          if (1.f > best[r] || (1.f == best[r] && t < pos[r])) { best[r] = 1.f; pos[r] = t; }
+        }
+      }
+    }
+    label[o] = best[r] > 0.5f ? ids[pos[r]] : -1;
+  }
+}
+
+int next_pow2(int v) {
+  int p = 64;
+  while (p < v) p <<= 1;
+  return p;
+}
+
+}  // namespace
+
+extern "C" int tfb200_track_masks_f32(const float* logits, const int32_t* src, const int32_t* ids,
+                                      const int32_t* prev_label, int32_t* label, int T, int h, int w, int size_h,
+                                      int size_w, int crop_h, int crop_w, int H, int W, void* stream) {
+  if (!src || !ids || !label) return TFB200_E_NULLPTR;
+  if (T < 0 || h <= 0 || w <= 0 || size_h <= 0 || size_w <= 0 || crop_h <= 0 || crop_w <= 0 || crop_h > size_h ||
+      crop_w > size_w || H <= 0 || W <= 0 || T > (1 << 24))
+    return TFB200_E_SHAPE;
+  if (T == 0) return 0;
+  const int hash_slots = prev_label ? next_pow2(2 * T) : 0;
+  const size_t smem = (size_t(2) * hash_slots + kMaxChunk) * sizeof(int) + kStageFloats * sizeof(float);
+  if (smem > size_t(kMaxSmem)) return TFB200_E_SHAPE;
+  if (smem > 48 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(track_masks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) return int(e);
+  }
+  const dim3 grid((W + kTileW - 1) / kTileW, (H + kTileH - 1) / kTileH);
+  track_masks_kernel<<<grid, kThreads, smem, cudaStream_t(stream)>>>(logits, src, ids, prev_label, label, T, h, w, size_h,
+                                                                     size_w, crop_h, crop_w, H, W, hash_slots);
+  msda_b200_count_launches(1);
+  return int(cudaGetLastError());
+}

@@ -540,7 +540,7 @@ TS_FN void ts_step(const TfbTrackStepArgs& a, Shared& sh) {
     o[1] = S.obj_ind[r];
     of[2] = S.score[r];
     of[3] = b.x0; of[4] = b.y0; of[5] = b.x1; of[6] = b.y1;
-    o[7] = 0;
+    o[7] = hs_src[r];                     // query row of this frame's embedding (and mask), or -1
   }
   TS_SYNC();
   if (tid == 0) {

@@ -14,6 +14,10 @@ track ids, `obj_ind`, `num_reids`, frame sets, boxes and scores.  What differs i
 
 CUDA only: on CPU tensors `step` raises (use `Tracker`, whose bookkeeping is host code by design).
 
+Segmentation masks work as in `Tracker`: word 7 of each result row is the query row whose embedding -- and so whose
+mask -- the track took this frame (-1: it keeps its previous mask), so the mask head runs on those rows after the
+read-back and the same resolution kernel writes the frame's label map.
+
 Differences a user can see: the debug logger receives the FRAME and INIT TRACK IDS lines only (the per-decision lines
 of tracker.py:375-379, 399-402, 232-235 would need the decisions on the host); `tracks` / `inactive_tracks` between
 frames cost one extra download of the state; tracks + object queries are limited to 2048 rows per frame.
@@ -74,6 +78,7 @@ class DeviceTracker(Tracker):
     def reset(self, hard=True):
         """tracker.py:71-80"""
         self._bufs = None
+        self._label = None
         self._cur = 0                                 # index of the state buffer holding the current state
         self._n_active = self._n_inactive = self._n_query = 0
         self._host_view = None
@@ -169,7 +174,8 @@ class DeviceTracker(Tracker):
             b = self._bufs
             target = [{"track_query_boxes": b["q_boxes"][:n_query], "image_id": b["image_id"],
                        "track_query_hs_embeds": b["q_embeds"][:n_query]}]
-        outputs, _, features, _, _ = self.obj_detector(img, target, self._prev_features[0])
+        det_out = self._detect(img, target, self._prev_features[0])
+        outputs, _, features, _, _ = det_out
         hs_embeds = outputs["hs_embed"][0].float().contiguous()
         rows = self._device_rows(outputs, orig_size).float().contiguous()
         nq = self.num_object_queries
@@ -221,9 +227,15 @@ class DeviceTracker(Tracker):
             raise RuntimeError(f"track_step kernel reported error {error} (1: query count / state mismatch, 2: capacity)")
         body = out[8:8 + 8 * n_results].reshape(n_results, 8)
         fbody = body.view(np.float32)
+        self._result_rows = body[:, 7].astype(np.int64)
+        label = None
+        if self.masks:
+            label = self._resolve_masks(det_out, self._result_rows, body[:, 0], blob, (height, width))
         for k in range(n_results):
-            self.results.setdefault(int(body[k, 0]), {})[self.frame_index] = {
-                "bbox": fbody[k, 3:7].copy(), "score": np.array(fbody[k, 2]), "obj_ind": int(body[k, 1])}
+            entry = {"bbox": fbody[k, 3:7].copy(), "score": np.array(fbody[k, 2]), "obj_ind": int(body[k, 1])}
+            if label is not None:
+                entry["mask"] = label == body[k, 0]
+            self.results.setdefault(int(body[k, 0]), {})[self.frame_index] = entry
         if track_num > self.track_num:
             self._logger(f"INIT TRACK IDS (detection_obj_score_thresh={self.detection_obj_score_thresh}): "
                          f"{list(range(self.track_num, track_num))}")

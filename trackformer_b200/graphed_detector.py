@@ -13,6 +13,10 @@ frame, so nothing about a frame's launch sequence is reusable as it stands.  `Gr
 
 It has the call signature, attributes and return value of the model it wraps -- `Tracker(GraphedDetector(model), ...)`
 -- except that `aux_outputs` are not returned (the tracker reads them only for verbose logging).
+
+For segmentation models (those with `detect` / `mask_logits`, segmentation.py) the graph holds `detect`, the forward
+without the mask head, so `pred_masks` is not returned either; `mask_logits(rows)` runs the head eagerly on the rows
+the tracker asks for, from the static buffers of the last call.
 `use_graphs=False` keeps the padding but runs the model eagerly (used by the CPU tests of the padding logic).
 """
 import torch
@@ -39,7 +43,9 @@ class GraphedDetector:
         # models that read prev_features (deformable_detr.py `_project_levels`): multi-frame attention and/or merged
         # frame features -- both must see the caller's previous-frame maps, and both keep what we return across frames
         self.uses_prev = self.multi_frame or bool(getattr(model, "merge_frame_features", False))
+        self.has_mask_head = callable(getattr(model, "mask_logits", None))
         self._plans = {}
+        self._last = None
         self.replays = 0
         self.captures = 0
 
@@ -72,8 +78,9 @@ class GraphedDetector:
         if plan.kb:
             targets = [{"track_query_boxes": plan.boxes, "track_query_hs_embeds": plan.hs,
                         "track_query_padding": plan.padding, "image_id": plan.image_id}]
+        forward = self.model.detect if self.has_mask_head else self.model
         with torch.no_grad():
-            out, _, plan.features, plan.memory, plan.hs_all = self.model(plan.img, targets, plan.prev)
+            out, _, plan.features, plan.memory, plan.hs_all = forward(plan.img, targets, plan.prev)
         plan.logits, plan.out_boxes, plan.hs_embed = out["pred_logits"], out["pred_boxes"], out["hs_embed"]
 
     def _build(self, key, img, kb, prev_features):
@@ -114,6 +121,7 @@ class GraphedDetector:
         return plan
 
     def __call__(self, samples, targets=None, prev_features=None):
+        self._last = None
         if isinstance(samples, NestedTensor) or not torch.is_tensor(samples) or samples.ndim != 4 or samples.shape[0] != 1:
             return self.model(samples, targets, prev_features)        # padded batches: outside the graphed domain
         k = 0
@@ -141,6 +149,7 @@ class GraphedDetector:
             self._run(plan)
 
         nq = self.num_queries
+        self._last = (plan, k)
 
         def real_rows(x, dim):
             """drop the filler rows kb-k ... : [track queries (k) | object queries (nq)]"""
@@ -161,3 +170,20 @@ class GraphedDetector:
         # NB: for models that never read prev_features the returned `features` / `memory` (and, when no filler rows had
         # to be dropped, the output rows) are views of the graph's static buffers: valid until the next call.
         return out, targets, features, plan.memory, real_rows(plan.hs_all, 2)
+
+    def detect(self, samples, targets=None, prev_features=None):
+        """The call itself: for segmentation models the graph already holds the forward without the mask head."""
+        return self(samples, targets, prev_features)
+
+    def mask_logits(self, rows):
+        """Mask logits ``[1, len(rows), H/4, W/4]`` of the real query rows ``rows`` of the last call ([track queries |
+        object queries], as returned), computed eagerly from the static feature / memory / decoder buffers.  Valid
+        until the next call."""
+        if not self.has_mask_head:
+            raise RuntimeError("GraphedDetector.mask_logits: the wrapped model has no mask head")
+        if self._last is None:
+            raise RuntimeError("GraphedDetector.mask_logits: no graphed call to take the rows from")
+        plan, k = self._last
+        padded = [int(r) if r < k else int(r) - k + plan.kb for r in rows]      # skip the filler rows k ... kb-1
+        with torch.no_grad():
+            return self.model.mask_logits(plan.features, plan.memory, plan.hs_all, padded)

@@ -218,8 +218,18 @@ class DETRSegmBase(nn.Module):
         self.mask_head = MaskHeadSmallConv(self.hidden_dim + nheads, self.fpn_channels, self.hidden_dim)
 
     def forward(self, samples: NestedTensor, targets: list = None, prev_features=None):
-        out, targets, features, memory, hs = super().forward(samples, targets, prev_features)
+        out, targets, features, memory, hs = self.detect(samples, targets, prev_features)
+        out["pred_masks"] = self.mask_logits(features, memory, hs)
+        return out, targets, features, memory, hs
 
+    def detect(self, samples: NestedTensor, targets: list = None, prev_features=None):
+        """The detection forward without the mask head: ``forward``'s return value without ``pred_masks``."""
+        return super().forward(samples, targets, prev_features)
+
+    def mask_logits(self, features, memory, hs, rows=None) -> Tensor:
+        """Mask logits ``[B, len(rows), H/4, W/4]`` of the query rows ``rows`` (all rows if None) from the outputs of
+        ``detect``.  Every query has its own attention softmax and its own GroupNorm sample, so a row's logits do not
+        depend on which other rows are computed with it."""
         src, mask = features[-2].decompose()                     # stride 16 (layer3)
         batch_size = src.shape[0]
         src = self.input_proj[-3](src)
@@ -227,10 +237,12 @@ class DETRSegmBase(nn.Module):
             mask = F.interpolate(mask[None].float(), size=src.shape[-2:]).to(torch.bool)[0]
         fpns = [features[-2].tensors, features[-3].tensors, features[-4].tensors]
 
-        bbox_mask = self.bbox_attention(hs[-1], memory[-3], mask=mask)
+        q = hs[-1]
+        if rows is not None:
+            q = q.index_select(1, torch.as_tensor(rows, dtype=torch.long, device=q.device))
+        bbox_mask = self.bbox_attention(q, memory[-3], mask=mask)
         seg_masks = self.mask_head(src, bbox_mask, fpns)
-        out["pred_masks"] = seg_masks.view(batch_size, hs.shape[2], seg_masks.shape[-2], seg_masks.shape[-1])
-        return out, targets, features, memory, hs
+        return seg_masks.view(batch_size, q.shape[1], seg_masks.shape[-2], seg_masks.shape[-1])
 
 
 class DeformableDETRSegm(DETRSegmBase, DeformableDETR):
@@ -244,6 +256,41 @@ class DeformableDETRSegmTracking(DETRSegmBase, DETRTrackingBase, DeformableDETR)
         DeformableDETR.__init__(self, **detr_kwargs)
         DETRTrackingBase.__init__(self, **tracking_kwargs)
         DETRSegmBase.__init__(self, **mask_kwargs)
+
+
+def resolve_track_masks(logits: Tensor, src, ids, prev_label: Optional[Tensor], size, crop, orig) -> Tensor:
+    """The online tracker's masks of one frame as a label map ``[H, W]`` int32 (track id, -1 for background).
+
+    ``ids`` are the active tracks in list order; ``src[t]`` is the row of ``logits`` ``[K, h, w]`` (stride-4 mask
+    logits) whose mask track ``t`` takes this frame, or -1 for a track that keeps its previous mask
+    ``prev_label == ids[t]``.  Same values as the reference: ``PostProcessSegm(return_probs=True)`` (bilinear to
+    ``size``, sigmoid, crop to ``crop``, nearest to ``orig``), stacked with the kept boolean masks as 0 / 1, and every
+    pixel labelled with the first track of maximal value if that value exceeds 0.5 (models/tracker.py:509-521).
+
+    On CUDA fp32 logits this is one launch of csrc/track_masks.cu; otherwise the reference's torch ops."""
+    H, W = (int(v) for v in orig)
+    src = torch.as_tensor(src, dtype=torch.int32).reshape(-1)
+    ids = torch.as_tensor(ids, dtype=torch.int32).reshape(-1)
+    dev = logits.device
+    if logits.is_cuda and logits.dtype == torch.float32:
+        prev = None if prev_label is None else prev_label.to(device=dev, dtype=torch.int32)
+        return ext.load().track_masks(logits.contiguous(), src.to(dev), ids.to(dev), prev, int(size[0]), int(size[1]),
+                                      int(crop[0]), int(crop[1]), H, W)
+    if len(ids) == 0:
+        return torch.full((H, W), -1, dtype=torch.int32, device=dev)
+    fresh = src >= 0
+    probs = torch.empty(len(ids), H, W, dtype=torch.float32, device=dev)
+    if bool(fresh.any()):
+        rows = logits.index_select(0, src[fresh].long().to(dev))
+        p = F.interpolate(rows[None].float(), size=(int(size[0]), int(size[1])), mode="bilinear", align_corners=False)
+        p = p.sigmoid()[0, :, :int(crop[0]), :int(crop[1])].unsqueeze(1)
+        probs[fresh.to(dev)] = F.interpolate(p, size=(H, W), mode="nearest")[:, 0]
+    if not bool(fresh.all()):
+        stale_ids = ids[~fresh].to(dev)
+        probs[(~fresh).to(dev)] = (prev_label.to(dev)[None] == stale_ids[:, None, None]).float()
+    arg = probs.argmax(0)
+    keep = probs.gather(0, arg[None])[0] > 0.5
+    return torch.where(keep, ids.to(dev)[arg], torch.full_like(arg, -1, dtype=torch.int32)).to(torch.int32)
 
 
 class PostProcessSegm(nn.Module):

@@ -18,6 +18,17 @@ the per-target state is a struct of arrays:
 
 All decisions are then taken on those host arrays in fp32, in the reference's order, so track ids, `obj_ind`,
 `num_reids` and the frame sets of the results are identical and boxes / scores are the detector's values bit for bit.
+
+Segmentation masks (MOTS, on when `obj_detector_post` has a "segm" entry; tracker.py:311-321, 333-373, 419-466,
+509-538).  The reference runs the mask head on every query row, upsamples every row to the image size, copies all of
+it to the host and then uses the few rows that end the frame as active tracks.  Here a track takes a new mask exactly
+where it takes a new embedding (`hs_writes`), so after the decisions the mask head runs on those rows only
+(`mask_logits` of a segmentation model, or `GraphedDetector.mask_logits`), and `resolve_track_masks`
+(csrc/track_masks.cu on the GPU) resolves the overlaps of all active tracks at the original resolution into one label
+map -- the frame's only extra read-back.  A track that keeps its previous mask reads it from the previous label map,
+which stays on the device.  `results[id][frame]["mask"]` is the reference's bool array [H, W]; `Track.mask` is the
+frame's resolved bool mask for active tracks and None for inactive ones (the reference keeps an inactive track's last
+mask, which nothing reads: a track that comes back always takes a new one).
 """
 from collections import deque
 
@@ -25,6 +36,9 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 from scipy.optimize import linear_sum_assignment
+
+from .graphed_detector import GraphedDetector
+from .segmentation import resolve_track_masks
 
 __all__ = ["Tracker", "Track", "nms_keep", "pairwise_iou"]
 
@@ -102,7 +116,7 @@ class Track:
         self.obj_ind = torch.tensor([int(s.obj_ind[slot])])
         self.hs_embed = [tracker._embedding_of(slot)]
         self.gt_id = None
-        self.mask = None
+        self.mask = tracker._mask_of(slot)
         self.attention_map = None
 
     def has_positive_area(self) -> bool:
@@ -155,8 +169,7 @@ class Tracker:
         if generate_attention_maps:
             # the reference asserts the same for the deformable model (tracker.py:38)
             raise ValueError("Generation of attention maps not possible for deformable DETR.")
-        if "segm" in obj_detector_post:
-            raise NotImplementedError("mask heads are outside the deformable tracking path")
+        self.masks = "segm" in obj_detector_post
         self.generate_attention_maps = False
         self._logger = logger if logger is not None else (lambda *log_strs: None)
         self._verbose = verbose
@@ -185,6 +198,7 @@ class Tracker:
 
     def reset(self, hard=True):
         """tracker.py:71-80"""
+        self._label = None                    # [H, W] int32 device label map of the last frame's masks
         self._state = _State()
         self._hs = None                       # [capacity, hidden] device embeddings, allocated at the first detection
         self._active, self._inactive = [], []
@@ -199,6 +213,52 @@ class Tracker:
     # ------------------------------------------------------------------------------------------------- internals
     def _embedding_of(self, slot):
         return self._hs[slot] if self._hs is not None else None
+
+    def _mask_of(self, slot):
+        if self._label is None or slot not in self._active:
+            return None
+        return self._label == int(self._state.ids[slot])
+
+    def _detect(self, img, target, prev_features):
+        """The detector call; with masks on, a segmentation model runs without its mask head (`detect`)."""
+        if self.masks and callable(getattr(self.obj_detector, "mask_logits", None)):
+            return self.obj_detector.detect(img, target, prev_features)
+        return self.obj_detector(img, target, prev_features)
+
+    def _mask_rows(self, det_out, rows):
+        """[len(rows), h, w] mask logits of the query rows `rows` of this frame's detector call."""
+        det = self.obj_detector
+        if isinstance(det, GraphedDetector):
+            return det.mask_logits(rows)[0]
+        if callable(getattr(det, "mask_logits", None)):
+            _, _, features, memory, hs = det_out
+            return det.mask_logits(features, memory, hs, rows)[0]
+        masks = det_out[0]["pred_masks"][0]           # any reference-shaped detector: the full head's output
+        return masks.index_select(0, torch.as_tensor(rows, dtype=torch.long, device=masks.device))
+
+    def _resolve_masks(self, det_out, src_rows, ids, blob, orig):
+        """Masks of the active tracks (ids, in list order) of this frame: `src_rows[t]` is the query row whose mask
+        track t takes, -1 to keep its previous one.  Returns the host label map [H, W] (the one read-back) or None."""
+        if not len(ids):
+            self._label = None
+            return None
+        stale = any(r < 0 for r in src_rows)
+        if stale and (self._label is None or tuple(self._label.shape) != tuple(orig)):
+            # the reference fails here too (torch.stack of masks of different sizes, tracker.py:510)
+            raise ValueError(f"orig_size changed to {tuple(orig)} while tracks keep their masks of size "
+                             f"{None if self._label is None else tuple(self._label.shape)}")
+        rows = sorted({int(r) for r in src_rows if r >= 0})
+        index = {r: i for i, r in enumerate(rows)}
+        src = [index[int(r)] if r >= 0 else -1 for r in src_rows]
+        if rows:
+            logits = self._mask_rows(det_out, rows)
+        else:
+            logits = torch.zeros(0, 1, 1, device=self._label.device)
+        size = [int(v) for v in blob["size"].reshape(-1, 2)[0].tolist()]
+        label = resolve_track_masks(logits, src, [int(i) for i in ids], self._label if stale else None, size, size,
+                                    orig)
+        self._label = label
+        return label.cpu().numpy()
 
     def _take_slot(self):
         if not self._free:
@@ -358,7 +418,8 @@ class Tracker:
                 "track_query_hs_embeds": self._hs.index_select(0, torch.as_tensor(order, device=dev)),
             }]
 
-        outputs, _, features, _, _ = self.obj_detector(img, target, self._prev_features[0])
+        det_out = self._detect(img, target, self._prev_features[0])
+        outputs, _, features, _, _ = det_out
         hs_embeds = outputs["hs_embed"][0]
         rows = self._packed_rows(outputs, orig_size)
         scores, labels = rows[:, 0], rows[:, 1]
@@ -447,11 +508,17 @@ class Tracker:
             self._active = [s for s, k in zip(self._active, ok) if k]
             released += dropped
 
-        # ---- results (tracker.py:533-548)
+        # ---- masks (tracker.py:509-521) and results (tracker.py:533-548)
+        self._result_rows = np.asarray([hs_writes.get(s, -1) for s in self._active], np.int64)
+        label = None
+        if self.masks:
+            label = self._resolve_masks(det_out, self._result_rows, st.ids[self._active], blob, (height, width))
         for s in self._active:
             box = st.pos[s] if self.obj_detector.overflow_boxes else _clip(st.pos[s], height, width)
-            self.results.setdefault(int(st.ids[s]), {})[self.frame_index] = {
-                "bbox": box.copy(), "score": np.array(st.score[s]), "obj_ind": int(st.obj_ind[s])}
+            entry = {"bbox": box.copy(), "score": np.array(st.score[s]), "obj_ind": int(st.obj_ind[s])}
+            if label is not None:
+                entry["mask"] = label == st.ids[s]
+            self.results.setdefault(int(st.ids[s]), {})[self.frame_index] = entry
         for s in self._inactive:
             st.count_inactive[s] += 1
         self.frame_index += 1
