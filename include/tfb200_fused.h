@@ -149,6 +149,23 @@ int tfb200_set_loss_fwd_f32(const float* logits, const float* boxes, const int64
                             const float* num_boxes, float* unit_logits, float* unit_l1, float* unit_giou, float* row_loss,
                             int* row_flags, float* pair_l1, float* pair_giou, float* out5k, int K, int B, int Q, int C,
                             int T, float alpha, float gamma, void* stream);
+/* Track-query training (models/matcher.py:112-128, models/detr_tracking.py):
+ *   match_cost_track : match_cost for logits / boxes [K][B][Q] with the forcing of row_pin [B*Q] (int32, the same for all
+ *                      K layers) applied in the same pass: -1 free row; c in [0, T) row pinned to global box c (its row
+ *                      is +inf except -1 at c; column c is +inf for every other row of the image); any other value an
+ *                      excluded row (all +inf: false-positive or filler track query).  T <= 49152.  Feeds tfb200_lsa_f32.
+ *   set_loss_fwd_masked: set_loss_fwd with row_valid [B*Q] (uint8, the same for all layers): a zero row adds nothing to
+ *                      loss_ce, is not counted by cardinality_error, has no pair terms and gets zero unit gradients (so
+ *                      set_loss_bwd gives it a zero gradient).                                                        */
+int tfb200_match_cost_track_f32(const float* logits, const float* boxes, const int64_t* tgt_ids, const float* tgt_boxes,
+                                const int* row_pin, float* cost, int K, int B, int Q, int C, int T, float w_class,
+                                float w_bbox, float w_giou, float alpha, float gamma, void* stream);
+int tfb200_set_loss_fwd_masked_f32(const float* logits, const float* boxes, const int64_t* src, const int64_t* tgt,
+                                   const int64_t* tgt_ids, const float* tgt_boxes, const int* offsets, const float* n_gt,
+                                   const float* num_boxes, const uint8_t* row_valid, float* unit_logits, float* unit_l1,
+                                   float* unit_giou, float* row_loss, int* row_flags, float* pair_l1, float* pair_giou,
+                                   float* out5k, int K, int B, int Q, int C, int T, float alpha, float gamma,
+                                   void* stream);
 int tfb200_set_loss_bwd_f32(const float* unit_logits, const float* unit_l1, const float* unit_giou, const float* g_ce,
                             const float* g_l1, const float* g_giou, const float* num_boxes, float* grad_logits,
                             float* grad_boxes, int K, int B, int Q, int C, void* stream);

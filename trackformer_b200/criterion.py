@@ -80,10 +80,14 @@ _FUSED_LOSS = os.environ.get("TFB200_FUSED_LOSS", "1") != "0"
 
 class _SetLoss(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets, n_gt, num_boxes, alpha, gamma):
+    def forward(ctx, logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets, n_gt, num_boxes, alpha, gamma, row_valid=None):
         from . import ext
-        out, ul, u1, ug = ext.load().set_loss_forward(logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets, n_gt,
-                                                      num_boxes, alpha, gamma)
+        if row_valid is None:
+            out, ul, u1, ug = ext.load().set_loss_forward(logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets, n_gt,
+                                                          num_boxes, alpha, gamma)
+        else:                                   # rows outside the mask (filler track queries) count for nothing
+            out, ul, u1, ug = ext.load().set_loss_forward_masked(logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets,
+                                                                 n_gt, num_boxes, row_valid, alpha, gamma)
         ctx.save_for_backward(ul, u1, ug, num_boxes)
         ce, l1, giou, card, cerr = out.unbind(0)
         ctx.mark_non_differentiable(card, cerr)
@@ -96,7 +100,7 @@ class _SetLoss(torch.autograd.Function):
         ul, u1, ug, num_boxes = ctx.saved_tensors
         gl, gb = ext.load().set_loss_backward(ul, u1, ug, g_ce.contiguous(), g_l1.contiguous(), g_giou.contiguous(),
                                               num_boxes)
-        return gl, gb, None, None, None, None, None, None, None, None, None
+        return gl, gb, None, None, None, None, None, None, None, None, None, None
 
 class LossDict(dict):
     """The loss dictionary of ``SetCriterion.forward_stacked`` (reference keys, detr.py:404-424) that also carries the
@@ -256,7 +260,7 @@ class SetCriterion(nn.Module):
             return out
         return t
 
-    def _fused_losses(self, logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes):
+    def _fused_losses(self, logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes, row_valid=None):
         """The loss values of ``forward_stacked`` and their gradients from three launches (csrc/set_loss.cu)."""
         k = logits.shape[0]
         dev = logits.device
@@ -273,7 +277,7 @@ class SetCriterion(nn.Module):
         tgt_boxes = torch.cat([t["boxes"] for t in targets]).float()
         ce, l1, gi, card, cerr = _SetLoss.apply(logits, boxes, src2d, tgt2d, tgt_ids, tgt_boxes, off, n_gt,
                                                 num_boxes.reshape(1).float(), float(self.focal_alpha),
-                                                float(self.focal_gamma))
+                                                float(self.focal_gamma), row_valid)
         losses = LossDict({"loss_ce": ce[-1], "class_error": cerr[-1], "loss_bbox": l1[-1], "loss_giou": gi[-1],
                            "cardinality_error": card[-1]})
         for i in range(k - 1):
@@ -284,20 +288,32 @@ class SetCriterion(nn.Module):
         losses.stacked = (ce, l1, gi)
         return losses
 
-    def forward_stacked(self, logits, boxes, targets, num_boxes=None, pred_masks=None):
+    def forward_stacked(self, logits, boxes, targets, num_boxes=None, pred_masks=None, track_queries=False):
         """Same losses as ``forward`` for a detector whose K decoder layers arrive stacked --
         ``logits [K,B,Q,C]``, ``boxes [K,B,Q,4]``, last layer = final prediction -- computed in ONE pass over
         all layers instead of K passes (the reference loops, detr.py:404-424): one Hungarian transfer, one focal
         loss, one L1/GIoU evaluation.  Keys and values equal ``forward`` on the equivalent dict (up to fp32
         summation order); falls back to it for the cases that need per-layer bookkeeping.  With the ``masks`` loss,
-        ``pred_masks [B,Q,h,w]`` of the last layer is scored against the last layer's matching."""
+        ``pred_masks [B,Q,h,w]`` of the last layer is scored against the last layer's matching.
+
+        ``track_queries=True`` opts tracking targets (``track_query_match_ids`` ...) into this pass instead of the
+        fallback: the track-query forcing of the matcher applies to every layer (on the device when it can, else on
+        the host), and ``track_query_padding [Kb]`` (True = filler row, as fed to the decoder) marks rows that are
+        neither matched nor scored -- they add nothing to any loss and get no gradient, and the focal loss is
+        normalised as in the unpadded model."""
         k, bs, nq, _ = logits.shape
         layers = [{"pred_logits": logits[i], "pred_boxes": boxes[i]} for i in range(k)]
         with_masks = "masks" in self.losses
         special = (not self.focal_loss or set(self.losses) - {"masks"} != {"labels", "boxes", "cardinality"}
-                   or any("track_query_match_ids" in t for t in targets) or not hasattr(self.matcher, "match_layers"))
+                   or not hasattr(self.matcher, "match_layers"))
+        forced = track_queries and any("track_query_match_ids" in t or "track_query_padding" in t for t in targets)
         sizes = [len(t["labels"]) for t in targets]
-        if special or min(sizes) == 0 or max(sizes) > nq:
+        if forced and (special or with_masks or not hasattr(self.matcher, "match_layers_forced")):
+            if any("track_query_padding" in t for t in targets):
+                raise NotImplementedError("filler track-query rows need the focal box-only criterion")
+            forced = False
+        if not forced and (special or any("track_query_match_ids" in t for t in targets)
+                           or min(sizes) == 0 or max(sizes) > nq):
             out = dict(layers[-1])
             if with_masks:
                 out["pred_masks"] = pred_masks
@@ -306,9 +322,17 @@ class SetCriterion(nn.Module):
 
         dev = logits.device
         per_layer = sum(sizes)
+        row_valid = None
+        if forced and any("track_query_padding" in t for t in targets):
+            row_valid = torch.stack([torch.cat([~t["track_query_padding"].to(dev),
+                                                torch.ones(nq - len(t["track_query_padding"]), dtype=torch.bool,
+                                                           device=dev)])
+                                     if "track_query_padding" in t else torch.ones(nq, dtype=torch.bool, device=dev)
+                                     for t in targets])                                          # [B, Q]
         device_match = None
         if self.device_matcher and hasattr(self.matcher, "match_layers_device"):
-            device_match = self.matcher.match_layers_device(logits.detach(), boxes.detach(), targets)
+            device_match = self.matcher.match_layers_device(logits.detach(), boxes.detach(), targets, forced=True) \
+                if forced else self.matcher.match_layers_device(logits.detach(), boxes.detach(), targets)
         if device_match is not None:
             # Hungarian matching on the device: no host synchronisation anywhere in the loss
             src2d, tgt2d, status = device_match
@@ -324,8 +348,11 @@ class SetCriterion(nn.Module):
             src, tgt = src2d.reshape(-1), tgt2d.reshape(-1)
             if num_boxes is None:               # callers replaying a captured step pass the (static) normaliser in
                 num_boxes = self._num_boxes(targets, dev)
+        elif forced:
+            all_indices = self.matcher.match_layers_forced(logits.detach(), boxes.detach(), targets)
         else:
             all_indices = self.matcher.match_layers(layers, targets)        # [K][B] (src, tgt) on the host
+        if device_match is None:
             if num_boxes is None:
                 num_boxes = self._num_boxes(targets, dev)
             lay = torch.arange(k).repeat_interleave(per_layer)
@@ -340,7 +367,8 @@ class SetCriterion(nn.Module):
             last = slice((k - 1) * per_layer, None)
             masks = mask_losses(pred_masks, bat[last] * nq + src[last], tgt[last], targets, num_boxes)
         if device_match is not None and _FUSED_LOSS and logits.dtype == torch.float32:
-            losses = self._fused_losses(logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes)
+            losses = self._fused_losses(logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes,
+                                        None if row_valid is None else row_valid.reshape(-1).to(torch.uint8))
             if with_masks:
                 losses.update(masks)
             return losses
@@ -359,6 +387,8 @@ class SetCriterion(nn.Module):
         focal = ce * ((1 - p_t) ** self.focal_gamma)
         if self.focal_alpha >= 0:
             focal = (self.focal_alpha * onehot + (1 - self.focal_alpha) * (1 - onehot)) * focal
+        if row_valid is not None:
+            focal = focal * row_valid[None, :, :, None].to(focal.dtype)
         loss_ce = focal.mean(2).sum((1, 2)) / num_boxes * nq                                   # [K]
 
         # boxes: L1 + GIoU over the matched pairs of every layer
@@ -368,7 +398,10 @@ class SetCriterion(nn.Module):
         loss_giou = (1 - giou).view(k, per_layer).sum(1) / num_boxes
 
         with torch.no_grad():
-            n_pred = (logits.argmax(-1) != logits.shape[-1] - 1).sum(2).float()                  # [K,B]
+            predicted = logits.argmax(-1) != logits.shape[-1] - 1
+            if row_valid is not None:
+                predicted = predicted & row_valid[None]
+            n_pred = predicted.sum(2).float()                                                    # [K,B]
             card = (n_pred - n_gt[None]).abs().mean(1)                                           # [K]
             last = slice((k - 1) * per_layer, None)
             class_error = 100 - accuracy(logits[-1][bat[last], src[last]], gt_labels[last])[0]

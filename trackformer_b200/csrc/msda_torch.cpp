@@ -621,6 +621,61 @@ std::vector<at::Tensor> set_loss_forward(const at::Tensor& logits, const at::Ten
   return {out, ul, u1, ug};
 }
 
+// logits [K,B,Q,C], boxes [K,B,Q,4], row_pin int32 [B*Q] -> cost [K,B,Q,T] with the track-query forcing applied
+at::Tensor match_cost_track(const at::Tensor& logits, const at::Tensor& boxes, const at::Tensor& tgt_ids,
+                            const at::Tensor& tgt_boxes, const at::Tensor& row_pin, double w_class, double w_bbox,
+                            double w_giou, double alpha, double gamma) {
+  TORCH_CHECK(logits.is_cuda() && boxes.is_cuda() && tgt_ids.is_cuda() && tgt_boxes.is_cuda() && row_pin.is_cuda(),
+              "match_cost_track: CUDA tensors expected");
+  TORCH_CHECK(logits.scalar_type() == at::kFloat && boxes.scalar_type() == at::kFloat && tgt_ids.scalar_type() == at::kLong &&
+              tgt_boxes.scalar_type() == at::kFloat && row_pin.scalar_type() == at::kInt, "match_cost_track: dtypes");
+  TORCH_CHECK(logits.dim() == 4 && boxes.dim() == 4, "match_cost_track: logits / boxes must be [K,B,Q,.]");
+  const at::Tensor lg = logits.contiguous(), bx = boxes.contiguous(), ti = tgt_ids.contiguous(), tb = tgt_boxes.contiguous();
+  const at::Tensor pin = row_pin.contiguous();
+  const int64_t K = lg.size(0), B = lg.size(1), Q = lg.size(2), C = lg.size(3), T = ti.numel();
+  TORCH_CHECK(bx.size(0) == K && bx.size(1) == B && bx.size(2) == Q && bx.size(3) == 4 && tb.numel() == T * 4 && T > 0 &&
+              pin.numel() == B * Q, "match_cost_track: shapes");
+  const c10::cuda::CUDAGuard guard(logits.device());
+  at::Tensor cost = at::empty({K, B, Q, T}, lg.options());
+  const int rc = tfb200_match_cost_track_f32(lg.data_ptr<float>(), bx.data_ptr<float>(), ti.data_ptr<int64_t>(),
+                                             tb.data_ptr<float>(), pin.data_ptr<int>(), cost.data_ptr<float>(), int(K),
+                                             int(B), int(Q), int(C), int(T), float(w_class), float(w_bbox), float(w_giou),
+                                             float(alpha), float(gamma), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "match_cost_track failed (code ", rc, ")");
+  return cost;
+}
+
+// set_loss_forward with a per-row validity mask row_valid uint8 [B*Q] (filler track queries = 0)
+std::vector<at::Tensor> set_loss_forward_masked(const at::Tensor& logits, const at::Tensor& boxes, const at::Tensor& src,
+                                                const at::Tensor& tgt, const at::Tensor& tgt_ids, const at::Tensor& tgt_boxes,
+                                                const at::Tensor& offsets, const at::Tensor& n_gt, const at::Tensor& num_boxes,
+                                                const at::Tensor& row_valid, double alpha, double gamma) {
+  TORCH_CHECK(logits.is_cuda() && logits.dim() == 4 && boxes.dim() == 4 && logits.scalar_type() == at::kFloat &&
+              boxes.scalar_type() == at::kFloat && src.scalar_type() == at::kLong && tgt.scalar_type() == at::kLong &&
+              tgt_ids.scalar_type() == at::kLong && tgt_boxes.scalar_type() == at::kFloat &&
+              offsets.scalar_type() == at::kInt && n_gt.scalar_type() == at::kFloat && num_boxes.scalar_type() == at::kFloat &&
+              row_valid.scalar_type() == at::kByte && num_boxes.is_cuda() && n_gt.is_cuda() && offsets.is_cuda() &&
+              row_valid.is_cuda(), "set_loss_forward_masked: dtypes / devices");
+  const at::Tensor lg = logits.contiguous(), bx = boxes.contiguous(), s = src.contiguous(), t = tgt.contiguous();
+  const at::Tensor ti = tgt_ids.contiguous(), tb = tgt_boxes.contiguous(), rv = row_valid.contiguous();
+  const int64_t K = lg.size(0), B = lg.size(1), Q = lg.size(2), C = lg.size(3), T = s.size(-1);
+  TORCH_CHECK(s.numel() == K * T && t.numel() == K * T && ti.numel() == T && tb.numel() == 4 * T && offsets.numel() == B + 1 &&
+              n_gt.numel() == B && rv.numel() == B * Q, "set_loss_forward_masked: shapes");
+  const c10::cuda::CUDAGuard guard(logits.device());
+  at::Tensor out = at::empty({5, K}, lg.options());
+  at::Tensor ul = at::empty_like(lg), u1 = at::empty_like(bx), ug = at::empty_like(bx);
+  at::Tensor row_loss = at::empty({K * B * Q}, lg.options()), row_flags = at::empty({K * B * Q}, lg.options().dtype(at::kInt));
+  at::Tensor pl = at::zeros({K, T}, lg.options()), pg = at::zeros({K, T}, lg.options());
+  const int rc = tfb200_set_loss_fwd_masked_f32(
+      lg.data_ptr<float>(), bx.data_ptr<float>(), s.data_ptr<int64_t>(), t.data_ptr<int64_t>(), ti.data_ptr<int64_t>(),
+      tb.data_ptr<float>(), offsets.data_ptr<int>(), n_gt.data_ptr<float>(), num_boxes.data_ptr<float>(),
+      rv.data_ptr<uint8_t>(), ul.data_ptr<float>(), u1.data_ptr<float>(), ug.data_ptr<float>(), row_loss.data_ptr<float>(),
+      row_flags.data_ptr<int>(), pl.data_ptr<float>(), pg.data_ptr<float>(), out.data_ptr<float>(), int(K), int(B), int(Q),
+      int(C), int(T), float(alpha), float(gamma), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "set_loss_forward_masked failed (code ", rc, ")");
+  return {out, ul, u1, ug};
+}
+
 std::vector<at::Tensor> set_loss_backward(const at::Tensor& unit_logits, const at::Tensor& unit_l1, const at::Tensor& unit_giou,
                                           const at::Tensor& g_ce, const at::Tensor& g_l1, const at::Tensor& g_giou,
                                           const at::Tensor& num_boxes) {
@@ -1034,6 +1089,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("match_cost", &match_cost);
   m.def("set_loss_forward", &set_loss_forward);
   m.def("set_loss_backward", &set_loss_backward);
+  m.def("match_cost_track", &match_cost_track);
+  m.def("set_loss_forward_masked", &set_loss_forward_masked);
   m.def("sampling_prep_forward", &sampling_prep_forward);
   m.def("sampling_prep_backward", &sampling_prep_backward);
   m.def("small_attention_forward", &small_attention_forward);

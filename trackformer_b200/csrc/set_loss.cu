@@ -6,9 +6,11 @@
 // one of them launch-bound on [6, N, 300, 91] / [6, 20, 4] tensors.  Same arithmetic here:
 //
 //   match_cost      cost[r][t] = w_bbox * |b_r - g_t|_1 + w_class * (pos - neg)(sigmoid(logit[r][label_t])) - w_giou * GIoU
+//                   (match_cost_track: the same, with track queries pinned to their identity's box, matcher.py:112-128)
 //   set_loss_rows   one warp per (layer, image, query) row: sigmoid focal loss of the row against its matched label
 //                   (none = all zeros), its gradient, the row's arg-max (cardinality / class error); the matched rows also
-//                   get the L1 and GIoU terms of their pair and the gradients of both with respect to the box
+//                   get the L1 and GIoU terms of their pair and the gradients of both with respect to the box; rows
+//                   outside the optional validity mask (filler track queries) contribute nothing and get zero gradients
 //   set_loss_final  one CTA per layer: fixed-order sums -> loss_ce / loss_bbox / loss_giou / cardinality_error (+ the
 //                   class error of the last layer), all divided by the device-resident normaliser num_boxes
 //   set_loss_bwd    grad_logits / grad_boxes from the three incoming gradient vectors [layers]
@@ -39,6 +41,19 @@ __device__ __forceinline__ float giou_value(const Box a, const Box g) {
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 
 // ---- matching cost (focal class cost; matcher.py:60-75) ------------------------------------------------------------
+__device__ __forceinline__ float match_cost_at(const float* __restrict__ logits, const float* __restrict__ boxes,
+                                               const int64_t* __restrict__ tgt_ids, const float* __restrict__ tgt_boxes,
+                                               int64_t r, int t, int C, float w_class, float w_bbox, float w_giou,
+                                               float alpha, float gamma) {
+  const float p = sigmoidf_(__ldg(logits + r * C + __ldg(tgt_ids + t)));
+  const float neg = (1.f - alpha) * powf(p, gamma) * (-logf(1.f - p + 1e-8f));
+  const float pos = alpha * powf(1.f - p, gamma) * (-logf(p + 1e-8f));
+  const float4 b = __ldg(reinterpret_cast<const float4*>(boxes) + r);
+  const float4 g = __ldg(reinterpret_cast<const float4*>(tgt_boxes) + t);
+  const float l1 = fabsf(b.x - g.x) + fabsf(b.y - g.y) + fabsf(b.z - g.z) + fabsf(b.w - g.w);
+  return w_bbox * l1 + w_class * (pos - neg) + w_giou * (-giou_value(to_xyxy(b), to_xyxy(g)));
+}
+
 __global__ void __launch_bounds__(256)
 match_cost_kernel(const float* __restrict__ logits, const float* __restrict__ boxes, const int64_t* __restrict__ tgt_ids,
                   const float* __restrict__ tgt_boxes, float* __restrict__ cost, int64_t R, int C, int T, float w_class,
@@ -47,13 +62,45 @@ match_cost_kernel(const float* __restrict__ logits, const float* __restrict__ bo
   if (i >= R * T) return;
   const int64_t r = i / T;
   const int t = int(i - r * T);
-  const float p = sigmoidf_(__ldg(logits + r * C + __ldg(tgt_ids + t)));
-  const float neg = (1.f - alpha) * powf(p, gamma) * (-logf(1.f - p + 1e-8f));
-  const float pos = alpha * powf(1.f - p, gamma) * (-logf(p + 1e-8f));
-  const float4 b = __ldg(reinterpret_cast<const float4*>(boxes) + r);
-  const float4 g = __ldg(reinterpret_cast<const float4*>(tgt_boxes) + t);
-  const float l1 = fabsf(b.x - g.x) + fabsf(b.y - g.y) + fabsf(b.z - g.z) + fabsf(b.w - g.w);
-  cost[i] = w_bbox * l1 + w_class * (pos - neg) + w_giou * (-giou_value(to_xyxy(b), to_xyxy(g)));
+  cost[i] = match_cost_at(logits, boxes, tgt_ids, tgt_boxes, r, t, C, w_class, w_bbox, w_giou, alpha, gamma);
+}
+
+// The same cost with the track-query rewrite of matcher.py:112-128 applied in the same pass.  row_pin [B*Q] (shared by
+// all layers): -1 free row; c in [0, T) row pinned to global box c (its row becomes +inf except -1 at c, and column c
+// becomes +inf for every other row of the image); any other value excluded row (all +inf: false-positive or filler
+// track query).  One CTA per (layer, image, kTrackRows rows); it first marks the image's pinned columns in shared memory.
+constexpr int kTrackRows = 16;
+
+__global__ void __launch_bounds__(256)
+match_cost_track_kernel(const float* __restrict__ logits, const float* __restrict__ boxes,
+                        const int64_t* __restrict__ tgt_ids, const float* __restrict__ tgt_boxes,
+                        const int* __restrict__ row_pin, float* __restrict__ cost, int B, int Q, int C, int T,
+                        float w_class, float w_bbox, float w_giou, float alpha, float gamma) {
+  extern __shared__ unsigned char col_pinned[];                      // [T]
+  const int chunks = (Q + kTrackRows - 1) / kTrackRows;
+  const int chunk = int(blockIdx.x % unsigned(chunks));
+  const int64_t kb = blockIdx.x / unsigned(chunks);                  // layer * B + image
+  const int b = int(kb % B);
+  const int* pin_b = row_pin + int64_t(b) * Q;
+  for (int t = threadIdx.x; t < T; t += blockDim.x) col_pinned[t] = 0;
+  __syncthreads();
+  for (int q = threadIdx.x; q < Q; q += blockDim.x) {
+    const int p = __ldg(pin_b + q);
+    if (p >= 0 && p < T) col_pinned[p] = 1;
+  }
+  __syncthreads();
+  const int q0 = chunk * kTrackRows;
+  const int rows = min(kTrackRows, Q - q0);
+  for (int i = threadIdx.x; i < rows * T; i += blockDim.x) {
+    const int q = q0 + i / T, t = i % T;
+    const int64_t r = kb * Q + q;
+    const int pin = __ldg(pin_b + q);
+    float v;
+    if (pin >= 0 && pin < T) v = t == pin ? -1.f : INFINITY;
+    else if (pin != -1 || col_pinned[t]) v = INFINITY;
+    else v = match_cost_at(logits, boxes, tgt_ids, tgt_boxes, r, t, C, w_class, w_bbox, w_giou, alpha, gamma);
+    cost[r * T + t] = v;
+  }
 }
 
 // ---- per-row loss terms and unit gradients ---------------------------------------------------------------------------
@@ -61,7 +108,8 @@ match_cost_kernel(const float* __restrict__ logits, const float* __restrict__ bo
 __global__ void __launch_bounds__(256)
 set_loss_rows_kernel(const float* __restrict__ logits, const float* __restrict__ boxes, const int64_t* __restrict__ src,
                      const int64_t* __restrict__ tgt, const int64_t* __restrict__ tgt_ids,
-                     const float* __restrict__ tgt_boxes, const int* __restrict__ off, float* __restrict__ unit_logits,
+                     const float* __restrict__ tgt_boxes, const int* __restrict__ off,
+                     const uint8_t* __restrict__ row_valid, float* __restrict__ unit_logits,
                      float* __restrict__ unit_l1, float* __restrict__ unit_giou, float* __restrict__ row_loss,
                      int* __restrict__ row_flags, float* __restrict__ pair_l1, float* __restrict__ pair_giou, int K,
                      int B, int Q, int C, int T, float alpha, float gamma) {
@@ -69,6 +117,17 @@ set_loss_rows_kernel(const float* __restrict__ logits, const float* __restrict__
   const int64_t r = int64_t(blockIdx.x) * 8 + (threadIdx.x >> 5);
   if (r >= int64_t(K) * B * Q) return;                               // warp-uniform
   const int q = int(r % Q), b = int((r / Q) % B), k = int(r / (int64_t(Q) * B));
+  if (row_valid != nullptr && !__ldg(row_valid + int64_t(b) * Q + q)) {
+    // masked row (filler track query): no loss, no cardinality count, zero unit gradients, no pair terms
+    for (int c = lane; c < C; c += 32) unit_logits[r * C + c] = 0.f;
+    if (lane == 0) {
+      row_loss[r] = 0.f;
+      row_flags[r] = 0;
+      reinterpret_cast<float4*>(unit_l1)[r] = make_float4(0.f, 0.f, 0.f, 0.f);
+      reinterpret_cast<float4*>(unit_giou)[r] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    return;                                                          // warp-uniform
+  }
 
   // which pair (if any) has this query as its source
   int hit = -1;
@@ -235,12 +294,28 @@ extern "C" int tfb200_match_cost_f32(const float* logits, const float* boxes, co
   return int(cudaGetLastError());
 }
 
-extern "C" int tfb200_set_loss_fwd_f32(const float* logits, const float* boxes, const int64_t* src, const int64_t* tgt,
-                                       const int64_t* tgt_ids, const float* tgt_boxes, const int* offsets,
-                                       const float* n_gt, const float* num_boxes, float* unit_logits, float* unit_l1,
-                                       float* unit_giou, float* row_loss, int* row_flags, float* pair_l1, float* pair_giou,
-                                       float* out5k, int K, int B, int Q, int C, int T, float alpha, float gamma,
-                                       void* stream) {
+extern "C" int tfb200_match_cost_track_f32(const float* logits, const float* boxes, const int64_t* tgt_ids,
+                                           const float* tgt_boxes, const int* row_pin, float* cost, int K, int B, int Q,
+                                           int C, int T, float w_class, float w_bbox, float w_giou, float alpha,
+                                           float gamma, void* stream) {
+  if (!logits || !boxes || !tgt_ids || !tgt_boxes || !row_pin || !cost) return TFB200_E_NULLPTR;
+  if (K < 0 || B <= 0 || Q <= 0 || C <= 0 || T <= 0 || T > 48 * 1024) return TFB200_E_SHAPE;
+  if (K == 0) return 0;
+  const int chunks = (Q + kTrackRows - 1) / kTrackRows;
+  const int64_t grid = int64_t(K) * B * chunks;
+  if (grid > 0x7fffffff) return TFB200_E_SHAPE;
+  match_cost_track_kernel<<<unsigned(grid), 256, size_t(T), cudaStream_t(stream)>>>(
+      logits, boxes, tgt_ids, tgt_boxes, row_pin, cost, B, Q, C, T, w_class, w_bbox, w_giou, alpha, gamma);
+  msda_b200_count_launches(1);
+  return int(cudaGetLastError());
+}
+
+namespace {
+int set_loss_fwd(const float* logits, const float* boxes, const int64_t* src, const int64_t* tgt, const int64_t* tgt_ids,
+                 const float* tgt_boxes, const int* offsets, const float* n_gt, const float* num_boxes,
+                 const uint8_t* row_valid, float* unit_logits, float* unit_l1, float* unit_giou, float* row_loss,
+                 int* row_flags, float* pair_l1, float* pair_giou, float* out5k, int K, int B, int Q, int C, int T,
+                 float alpha, float gamma, void* stream) {
   if (!logits || !boxes || !src || !tgt || !tgt_ids || !tgt_boxes || !offsets || !n_gt || !num_boxes || !unit_logits ||
       !unit_l1 || !unit_giou || !row_loss || !row_flags || !pair_l1 || !pair_giou || !out5k)
     return TFB200_E_NULLPTR;
@@ -248,11 +323,35 @@ extern "C" int tfb200_set_loss_fwd_f32(const float* logits, const float* boxes, 
   cudaStream_t st = cudaStream_t(stream);
   const int64_t R = int64_t(K) * B * Q;
   set_loss_rows_kernel<<<unsigned((R + 7) / 8), 256, 0, st>>>(logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets,
-                                                              unit_logits, unit_l1, unit_giou, row_loss, row_flags, pair_l1,
-                                                              pair_giou, K, B, Q, C, T, alpha, gamma);
+                                                              row_valid, unit_logits, unit_l1, unit_giou, row_loss,
+                                                              row_flags, pair_l1, pair_giou, K, B, Q, C, T, alpha, gamma);
   set_loss_final_kernel<<<K, 256, 0, st>>>(row_loss, row_flags, pair_l1, pair_giou, n_gt, num_boxes, out5k, K, B, Q, T);
   msda_b200_count_launches(2);
   return int(cudaGetLastError());
+}
+}  // namespace
+
+extern "C" int tfb200_set_loss_fwd_f32(const float* logits, const float* boxes, const int64_t* src, const int64_t* tgt,
+                                       const int64_t* tgt_ids, const float* tgt_boxes, const int* offsets,
+                                       const float* n_gt, const float* num_boxes, float* unit_logits, float* unit_l1,
+                                       float* unit_giou, float* row_loss, int* row_flags, float* pair_l1, float* pair_giou,
+                                       float* out5k, int K, int B, int Q, int C, int T, float alpha, float gamma,
+                                       void* stream) {
+  return set_loss_fwd(logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets, n_gt, num_boxes, nullptr, unit_logits, unit_l1,
+                      unit_giou, row_loss, row_flags, pair_l1, pair_giou, out5k, K, B, Q, C, T, alpha, gamma, stream);
+}
+
+extern "C" int tfb200_set_loss_fwd_masked_f32(const float* logits, const float* boxes, const int64_t* src,
+                                              const int64_t* tgt, const int64_t* tgt_ids, const float* tgt_boxes,
+                                              const int* offsets, const float* n_gt, const float* num_boxes,
+                                              const uint8_t* row_valid, float* unit_logits, float* unit_l1,
+                                              float* unit_giou, float* row_loss, int* row_flags, float* pair_l1,
+                                              float* pair_giou, float* out5k, int K, int B, int Q, int C, int T,
+                                              float alpha, float gamma, void* stream) {
+  if (!row_valid) return TFB200_E_NULLPTR;
+  return set_loss_fwd(logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets, n_gt, num_boxes, row_valid, unit_logits,
+                      unit_l1, unit_giou, row_loss, row_flags, pair_l1, pair_giou, out5k, K, B, Q, C, T, alpha, gamma,
+                      stream);
 }
 
 extern "C" int tfb200_set_loss_bwd_f32(const float* unit_logits, const float* unit_l1, const float* unit_giou,

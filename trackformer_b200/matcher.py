@@ -62,6 +62,11 @@ class HungarianMatcher(nn.Module):
         logits = torch.stack([o["pred_logits"] for o in outputs_list]).flatten(0, 2)
         boxes = torch.stack([o["pred_boxes"] for o in outputs_list]).flatten(0, 2)
         cost = self._cost(logits, boxes, tgt_ids, tgt_boxes).view(k, bs, nq, -1).cpu()
+        return self._assign(cost, sizes)
+
+    @staticmethod
+    def _assign(cost, sizes):
+        """scipy on every (layer, image) block of a host ``cost [K,B,Q,T]`` -> [K][B] (src, tgt)"""
         result = []
         for layer in cost:
             picks = [linear_sum_assignment(c[i]) for i, c in enumerate(layer.split(sizes, -1))]
@@ -69,22 +74,95 @@ class HungarianMatcher(nn.Module):
                            for r, c in picks])
         return result
 
+    @staticmethod
+    def row_pin(targets, num_rows, device):
+        """The track-query forcing of ``forward`` (:112-128) as one int32 code per (image, query row), ``[B * num_rows]``:
+        -1 free row, -2 excluded row (false-positive track query, or a filler row), c >= 0 row pinned to GLOBAL box
+        column c.  The k-th track row that is not a false positive takes ``track_query_match_ids[k]``, as in ``forward``.
+        ``track_query_padding [Kb]`` (bool, True = filler) lays the unpadded rows of the masks, in order, onto the
+        non-filler rows of a ``[Kb + object queries]`` layout.  Built on the device without reading anything back."""
+        pins, col0 = [], 0
+        for t in targets:
+            pad = t.get("track_query_padding")
+            if "track_query_match_ids" in t:
+                fal_pos = t["track_queries_fal_pos_mask"].to(device)
+                pinned = t["track_queries_mask"].to(device) & ~fal_pos
+                ids = t["track_query_match_ids"].to(device=device, dtype=torch.int64)
+                ids = torch.cat([ids, ids.new_zeros(1)])                 # keeps the gather defined when there are none
+                rank = (pinned.long().cumsum(0) - 1).clamp(min=0)
+                pin = torch.where(pinned, ids[rank] + col0, torch.full_like(rank, -1))
+                pin = torch.where(fal_pos, torch.full_like(pin, -2), pin)
+            else:
+                pin = torch.full((num_rows,), -1, dtype=torch.int64, device=device)      # (only the head is read)
+            if pad is not None:
+                real = torch.cat([~pad.to(device), torch.ones(num_rows - pad.shape[0], dtype=torch.bool, device=device)])
+                where = (real.long().cumsum(0) - 1).clamp(min=0)
+                pin = torch.where(real, pin[where], torch.full_like(where, -2))
+            pins.append(pin)
+            col0 += len(t["boxes"])
+        return torch.stack(pins).to(torch.int32).reshape(-1)
+
+    @staticmethod
+    def force_cost(cost, row_pin):
+        """``cost [..., B, Q, T]`` rewritten by ``row_pin [B*Q]`` (see ``row_pin``): the rewrite ``forward`` applies
+        (:112-128), in torch.  The device kernel (csrc/set_loss.cu, match_cost_track) applies the same one."""
+        bs, nq, n_cols = cost.shape[-3:]
+        pin = row_pin.to(cost.device, torch.int64).view(bs, nq)
+        pinned = (pin >= 0) & (pin < n_cols)
+        excluded = ~pinned & (pin != -1)
+        cols = torch.arange(n_cols, device=cost.device)
+        col_pinned = torch.zeros(bs, n_cols + 1, dtype=torch.bool, device=cost.device)
+        col_pinned.scatter_(1, torch.where(pinned, pin, n_cols), True)
+        col_pinned = col_pinned[:, :n_cols]
+        inf = torch.full((), float("inf"), dtype=cost.dtype, device=cost.device)
+        at_pin = torch.where(cols == pin[..., None], torch.full((), -1.0, dtype=cost.dtype, device=cost.device), inf)
+        blocked = excluded[..., None] | col_pinned[:, None, :]
+        return torch.where(pinned[..., None], at_pin, torch.where(blocked, inf, cost))
+
     @torch.no_grad()
-    def match_layers_device(self, logits, boxes, targets):
+    def match_layers_forced(self, logits, boxes, targets):
+        """Host route of the forced matching for stacked ``logits [K,B,Q,C]`` / ``boxes [K,B,Q,4]``: the rewrite of
+        ``row_pin`` / ``force_cost`` and scipy per layer and image -> [K][B] (src, tgt).  Unlike ``forward`` it accepts
+        filler rows (``track_query_padding``); on the real rows it gives ``forward``'s pairs."""
+        k, bs, nq, _ = logits.shape
+        sizes = [len(t["boxes"]) for t in targets]
+        if sum(sizes) == 0:
+            empty = torch.zeros(0, dtype=torch.int64)
+            return [[(empty, empty) for _ in range(bs)] for _ in range(k)]
+        tgt_ids = torch.cat([t["labels"] for t in targets])
+        tgt_boxes = torch.cat([t["boxes"] for t in targets])
+        cost = self._cost(logits.flatten(0, 2), boxes.flatten(0, 2), tgt_ids, tgt_boxes).view(k, bs, nq, -1)
+        cost = self.force_cost(cost, self.row_pin(targets, nq, logits.device)).cpu()
+        return self._assign(cost, sizes)
+
+    @torch.no_grad()
+    def match_layers_device(self, logits, boxes, targets, forced=False):
         """All K layers' matchings ON THE DEVICE (csrc/lsa.cu): no device->host transfer, CUDA-graph capturable.
         ``logits [K,B,Q,C]``, ``boxes [K,B,Q,4]`` -> ``(src [K,T], tgt [K,T], status)`` with T = total number of
         boxes; for image b the columns ``off[b]..off[b+1]-1`` hold its (query, box) pairs in ascending query order --
         the pairs scipy returns (the optimum is unique unless costs tie exactly).  Returns ``None`` when the device
-        solver does not apply (track-query forcing, more boxes than queries, CPU tensors)."""
+        solver does not apply (more boxes than queries, no boxes at all, CPU tensors) and, unless ``forced``, for
+        targets with track-query forcing.  With ``forced`` the track-query rewrite of ``forward`` (see ``row_pin``,
+        filler rows included) is applied to the cost of every layer in the same launch; an image without boxes then
+        takes the host route (``match_layers_forced``)."""
         from . import ext
         k, bs, nq, _ = logits.shape
         sizes = [len(t["boxes"]) for t in targets]
-        if (not logits.is_cuda or any("track_query_match_ids" in t for t in targets) or max(sizes) > nq
-                or sum(sizes) == 0):
+        if (not logits.is_cuda or (not forced and any("track_query_match_ids" in t for t in targets))
+                or max(sizes) > nq or sum(sizes) == 0 or (forced and min(sizes) == 0)):
             return None
         tgt_ids = torch.cat([t["labels"] for t in targets])
         tgt_boxes = torch.cat([t["boxes"] for t in targets])
-        if _FUSED_LOSS and self.focal_loss and logits.dtype == torch.float32:
+        fused = _FUSED_LOSS and self.focal_loss and logits.dtype == torch.float32
+        if forced:
+            pin = self.row_pin(targets, nq, logits.device)
+            if fused:
+                cost = ext.load().match_cost_track(logits, boxes, tgt_ids, tgt_boxes.float(), pin, self.cost_class,
+                                                   self.cost_bbox, self.cost_giou, self.focal_alpha, self.focal_gamma)
+            else:
+                cost = self._cost(logits.flatten(0, 2), boxes.flatten(0, 2), tgt_ids, tgt_boxes).view(k, bs, nq, -1)
+                cost = self.force_cost(cost, pin)
+        elif fused:
             # the whole cost matrix in one launch (csrc/set_loss.cu) instead of ~25 elementwise kernels
             cost = ext.load().match_cost(logits, boxes, tgt_ids, tgt_boxes.float(), self.cost_class, self.cost_bbox,
                                          self.cost_giou, self.focal_alpha, self.focal_gamma).view(k, bs, nq, -1)

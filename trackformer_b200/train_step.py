@@ -15,6 +15,11 @@ replayed -- two graph launches instead of thousands of kernel launches.  The bac
 accumulation into the gradient buffer, so nothing per-parameter runs eagerly.  Between the two sits what cannot be captured: the Hungarian matching (scipy on the host, like the
 reference, matcher.py:104,127 -- the index bookkeeping must stay bit-exact) and the loss, which is small.
 
+Tracking: for a ``DETRTrackingBase`` model in training mode whose targets carry ``prev_image`` / ``prev_target``, a step
+is the reference's tracking step (detr_tracking.py forward + criterion + backward), decomposed so that the heavy parts
+replay from graphs as well -- see ``_tracking_route`` for how a step's route is chosen and ``_track_step`` for the
+pieces.
+
 Multi-GPU: one process per GPU.  Gradients live in ONE flat fp32 buffer (every ``param.grad`` is a view into
 it), so the data-parallel exchange is a single NCCL all-reduce of 162 MB over NVLink/NVSwitch after the backward
 graph, followed by clip + fused AdamW.  (DDP's bucketed overlap would hide ~0.4 ms of a ~20 ms step; a single
@@ -39,6 +44,19 @@ class _DetectorCore(nn.Module):
 
     def forward(self, frames):
         out, _, _, _, _ = self.model(frames, None, None)
+        return self._heads(out)
+
+    def detector(self, frames, targets=None, prev_features=None):
+        """The detector's own forward (``DeformableDETR.forward``) of a tracking model: previous frames, and current
+        frames with precomputed track-query targets -- not ``DETRTrackingBase.forward``, which would rewrite them."""
+        from .detr_tracking import DETRTrackingBase
+        return super(DETRTrackingBase, self.model).forward(frames, targets, prev_features)
+
+    def track(self, frames, targets, prev_features):
+        out, _, _, _, _ = self.detector(frames, targets, prev_features)
+        return self._heads(out)
+
+    def _heads(self, out):
         stacked = getattr(self.model, "stacked_heads", None)
         if stacked is not None and stacked[0].shape[0] == len(out["aux_outputs"]) + 1:
             return stacked                           # the very tensors the dictionary entries are slices of
@@ -52,10 +70,16 @@ class TrainStep:
 
     def __init__(self, model, criterion, optimizer_factory=None, max_norm: float = 0.1,
                  use_graphs: bool = True, example_frames: Optional[torch.Tensor] = None,
-                 example_targets: Optional[list] = None, flat_adamw: Optional[dict] = None):
+                 example_targets: Optional[list] = None, flat_adamw: Optional[dict] = None, track_bucket: int = 32):
         """``optimizer_factory(params)`` builds any torch optimizer; ``flat_adamw={'groups': [...], 'betas':..., 'eps':...}``
         (groups as for torch.optim.AdamW, e.g. flat_adamw.reference_param_groups(model)) instead lays the PARAMETERS out
-        flat as well and updates them with the one-pass clip + AdamW kernel."""
+        flat as well and updates them with the one-pass clip + AdamW kernel.  ``track_bucket``: tracking steps pad their
+        track queries up to a multiple of it, and one pair of current-frame graphs is captured per padded count."""
+        if track_bucket < 1:
+            raise ValueError("track_bucket must be >= 1")
+        self.track_bucket = int(track_bucket)
+        self._prev_plans, self._track_plans = {}, {}
+        self.track_captures = 0
         if hasattr(model, "mask_head") or "masks" in getattr(criterion, "losses", ()):
             raise NotImplementedError("TrainStep does not train segmentation models (their mask losses would be "
                                       "dropped); run the model and SetCriterion eagerly instead")
@@ -341,9 +365,12 @@ class TrainStep:
             if g is None:
                 v.zero_()
 
-    def _loss(self, logits, boxes, targets, num_boxes=None):
+    def _loss(self, logits, boxes, targets, num_boxes=None, track_queries=False):
         """Weighted total of the criterion's entries (engine.py:139-140: sum(loss_dict[k] * weight_dict[k]))."""
-        loss_dict = self.criterion.forward_stacked(logits, boxes, targets, num_boxes)
+        if track_queries:
+            loss_dict = self.criterion.forward_stacked(logits, boxes, targets, num_boxes, track_queries=True)
+        else:
+            loss_dict = self.criterion.forward_stacked(logits, boxes, targets, num_boxes)
         wd = self.criterion.weight_dict
         stacked = getattr(loss_dict, "stacked", None)
         names = ("loss_ce", "loss_bbox", "loss_giou")
@@ -358,6 +385,193 @@ class TrainStep:
                 self._loss_w_key = key
             return (torch.stack(stacked) * self._loss_w).sum()
         return sum(loss_dict[k] * wd[k] for k in loss_dict if k in wd)
+
+    # ------------------------------------------------------------------------------------------ tracking
+    def _tracking_route(self, targets) -> str:
+        """How ``step(frames, targets)`` runs, decided by the model, the criterion and the targets:
+
+        ``"detect"``  the detection step: the model is not a tracking model in training mode, or the targets carry no
+                      ``prev_image`` (the tracking model then trains detection, as its own forward would);
+        ``"eager"``   the reference composition -- model(frames, targets) + ``criterion.forward`` + backward into the flat
+                      gradient -- for what the decomposed step does not cover: a previous-previous frame
+                      (``prev_prev_image``), backpropagation through the previous frame, and criteria other than the
+                      focal box-only one;
+        ``"track"``   everything else: the decomposed step of ``_track_step``."""
+        from .detr_tracking import DETRTrackingBase
+        model, crit = self.model, self.criterion
+        if (not isinstance(model, DETRTrackingBase) or not model.training or model._tracking or not targets
+                or "prev_image" not in targets[0]):
+            return "detect"
+        if ("prev_prev_image" in targets[0] or model._backprop_prev_frame or not crit.focal_loss
+                or set(crit.losses) != {"labels", "boxes", "cardinality"}
+                or not hasattr(crit.matcher, "match_layers_forced")):
+            return "eager"
+        return "track"
+
+    def _tracking_eager(self, frames, targets, num_boxes):
+        out, targets_out, _, _, _ = self.model(frames, targets)
+        loss_dict = self.criterion(out, targets_out, num_boxes)
+        wd = self.criterion.weight_dict
+        loss = sum(loss_dict[k] * wd[k] for k in loss_dict if k in wd)
+        self._backward_into_flat(loss)
+        return loss
+
+    def _graphs(self) -> bool:
+        return self.g_fwd is not None
+
+    def _warm_up_and_capture(self, run, backward: bool):
+        """Capture ``run`` (and, with ``backward``, the zero-fill + backward of its outputs) into graphs of the step's
+        pool.  The warm-up passes draw nothing from the CPU generator; its state is restored regardless, so that the
+        track-query decisions of a step do not depend on whether it captured."""
+        with torch.random.fork_rng(devices=[]):
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                for _ in range(2):
+                    outs = run()
+                    if backward:
+                        torch.autograd.backward(outs, [torch.zeros_like(o) for o in outs])
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            g_fwd = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g_fwd, pool=self._pool):
+                outs = run()
+            g_bwd = grads = None
+            if backward:
+                grads = [torch.zeros_like(o) for o in outs]
+                g_bwd = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g_bwd, pool=self._pool):
+                    self.flat_grad.zero_()
+                    torch.autograd.backward(outs, grads)
+                self.flat_grad.zero_()
+        self.track_captures += 1
+        return g_fwd, outs, g_bwd, grads
+
+    def _previous_frame(self, targets):
+        """Step 1: the previous frames through the detector under no_grad (training mode, as the reference runs them),
+        replayed from one graph per image shape.  -> (logits, boxes, hs_embed of the last layer, backbone features)."""
+        images = [t["prev_image"] for t in targets]
+        if not self._graphs() or len({tuple(im.shape) for im in images}) != 1:
+            with torch.no_grad():
+                out, _, features, _, _ = self.core.detector(images)
+            return out["pred_logits"], out["pred_boxes"], out["hs_embed"], features, None
+        frames = torch.stack(images)
+        key = (tuple(frames.shape), frames.dtype)
+        plan = self._prev_plans.get(key)
+        if plan is None:
+            plan = {"frames": frames.clone()}
+
+            def run():
+                with torch.no_grad():
+                    out, _, features, _, _ = self.core.detector(plan["frames"])
+                plan["features"] = features
+                return out["pred_logits"], out["pred_boxes"], out["hs_embed"]
+            plan["graph"], plan["outs"], _, _ = self._warm_up_and_capture(run, backward=False)
+            self._prev_plans[key] = plan
+        plan["frames"].copy_(frames)
+        plan["graph"].replay()
+        return (*plan["outs"], plan["features"], key)
+
+    def _previous_matching(self, logits, boxes, prev_targets):
+        """Step 2: the previous frame's last layer against its boxes, unforced -- what the model's own matcher computes
+        (detr_tracking.py) -- on the device, with the pairs read back once for the bookkeeping."""
+        matcher = self.model._matcher
+        sizes = [len(t["boxes"]) for t in prev_targets]
+        found = None
+        if logits.is_cuda and self.criterion.device_matcher and min(sizes) > 0:
+            found = matcher.match_layers_device(logits[None], boxes[None], prev_targets)
+        if found is None:
+            return matcher({"pred_logits": logits, "pred_boxes": boxes}, prev_targets)
+        src, tgt, status = found
+        host = torch.cat([src[0], tgt[0], status.long()]).cpu()
+        if int(host[-1]) != 0:
+            raise RuntimeError(f"device Hungarian matching failed (status {int(host[-1])})")
+        n = sum(sizes)
+        src_h, tgt_h = host[:n], host[n:2 * n]
+        out, ofs = [], 0
+        for size in sizes:
+            out.append((src_h[ofs:ofs + size].clone(), tgt_h[ofs:ofs + size] - ofs))
+            ofs += size
+        return out
+
+    def _track_step(self, frames, targets, num_boxes):
+        """The reference's tracking step (DETRTrackingBase.forward(samples, targets) + criterion + backward), in pieces:
+
+          1. previous frames, no_grad, from a graph per image shape (``_previous_frame``);
+          2. their matching on the device (``_previous_matching``);
+          3. the model's own ``add_track_queries_to_targets``, unchanged: the same decisions and the same CPU-generator
+             draws as the eager model -- the only host reads of the step (boxes, matched pairs, track ids) are here;
+          4. the current frame with the K track queries padded to a multiple of ``track_bucket`` (filler rows hidden
+             from the real queries by ``track_query_padding``), replayed from a forward and a backward graph per padded
+             count, with the forced device matching and the row-masked fused loss in between (``_track_current``).
+
+        Without graphs (``use_graphs=False``, or on the CPU) the same pieces run eagerly.
+
+        Memory: every captured current-frame bucket keeps its own forward activations alive in the shared pool (its
+        backward graph consumes them at replay), so each bucket costs about one forward's saved activations, plus one
+        previous-frame graph per image shape; the backward graphs' temporaries are shared.  A coarser ``track_bucket``
+        means fewer buckets."""
+        prev_targets = [t["prev_target"] for t in targets]
+        logits, boxes, hs, features, prev_key = self._previous_frame(targets)
+        prev_indices = self._previous_matching(logits, boxes, prev_targets)
+        self.model.add_track_queries_to_targets(targets, prev_indices, {"pred_boxes": boxes, "hs_embed": hs})
+        uses_prev = bool(getattr(self.model, "multi_frame_attention", False) or
+                         getattr(self.model, "merge_frame_features", False))
+        return self._track_current(frames, targets, num_boxes, features if uses_prev else None,
+                                   prev_key if uses_prev else None)
+
+    def _track_current(self, frames, targets, num_boxes, prev_features, prev_key):
+        """Step 4 of ``_track_step``: no host synchronisation from here to the end of the step."""
+        n_track = {int(t["track_query_boxes"].shape[0]) for t in targets}
+        if len(n_track) != 1:
+            raise ValueError("every image of a tracking batch needs the same number of track queries")
+        k = n_track.pop()
+        kb = 0 if k == 0 else -(-k // self.track_bucket) * self.track_bucket
+        padded = self.track_bucket > 1 and kb > 0
+        bs, dev = frames.shape[0], frames.device
+        dim = self.model.hidden_dim
+        # graphs read the previous frame's features from its graph's static buffers: none when that frame ran eagerly
+        graphed = self._graphs() and (prev_features is None or prev_key is not None)
+        key = (tuple(frames.shape), frames.dtype, kb, prev_key)
+        plan = self._track_plans.get(key) if graphed else None
+        new = plan is None
+        if new:
+            plan = {"frames": frames.clone() if graphed else frames, "hs": torch.zeros(bs, kb, dim, device=dev),
+                    "boxes": torch.full((bs, kb, 4), 0.5, device=dev),
+                    "padding": torch.zeros(bs, kb, dtype=torch.bool, device=dev), "slot": torch.arange(kb, device=dev)}
+            if graphed:
+                self._track_plans[key] = plan
+        elif plan["frames"] is not frames:
+            plan["frames"].copy_(frames, non_blocking=True)
+        track_targets = None
+        if kb:
+            plan["hs"][:, :k].copy_(torch.stack([t["track_query_hs_embeds"] for t in targets]))
+            plan["boxes"][:, :k].copy_(torch.stack([t["track_query_boxes"] for t in targets]))
+            plan["padding"].copy_((plan["slot"] >= k).expand(bs, kb))
+            track_targets = [{"track_query_hs_embeds": plan["hs"][b], "track_query_boxes": plan["boxes"][b]}
+                             for b in range(bs)]
+            if padded:
+                for b, tt in enumerate(track_targets):
+                    tt["track_query_padding"] = plan["padding"][b]
+        loss_targets = [dict(t, track_query_padding=plan["padding"][b]) if padded else t for b, t in enumerate(targets)]
+
+        def run():
+            return self.core.track(plan["frames"], track_targets, prev_features)
+
+        if not graphed:
+            logits, boxes = run()
+            loss = self._loss(logits, boxes, loss_targets, num_boxes, track_queries=True)
+            self._backward_into_flat(loss)
+            return loss
+        if new:
+            plan["g_fwd"], plan["outs"], plan["g_bwd"], plan["grads"] = self._warm_up_and_capture(run, backward=True)
+        plan["g_fwd"].replay()
+        logits, boxes = (o.detach().requires_grad_(True) for o in plan["outs"])
+        loss = self._loss(logits, boxes, loss_targets, num_boxes, track_queries=True)
+        for dst, g in zip(plan["grads"], torch.autograd.grad(loss, (logits, boxes))):
+            dst.copy_(g)
+        plan["g_bwd"].replay()
+        return loss
 
     def _normaliser(self, targets, device):
         if self.s_num_boxes is None:
@@ -400,11 +614,15 @@ class TrainStep:
             frames, self._staged = self._staged, None
             if dev.type == "cuda":
                 torch.cuda.current_stream(dev).wait_event(self._staged_ready)
-        full = self.g_full is not None and tuple(len(t["labels"]) for t in targets) == self.full_sizes
+        route = self._tracking_route(targets)
+        full = (route == "detect" and self.g_full is not None
+                and tuple(len(t["labels"]) for t in targets) == self.full_sizes)
         # one scalar all-reduce per step on EVERY path, before anything else (same collective order on all ranks)
-        num_boxes = self._normaliser(targets, dev) if (self.world > 1 or full) else None
+        num_boxes = self._normaliser(targets, dev) if (self.world > 1 or full or route == "track") else None
         pending = None
-        if full:
+        if route != "detect":
+            loss = (self._track_step if route == "track" else self._tracking_eager)(frames, targets, num_boxes)
+        elif full:
             if frames is not self.static_frames:
                 self.static_frames.copy_(frames, non_blocking=True)     # device or pinned-host source
             if staged and dev.type == "cuda":
