@@ -241,9 +241,10 @@ int tfb200_track_step_f32(const TfbTrackStepArgs* args, void* stream);
  * N = images * per_image; an operand "per image" is [N / per_image][...] and is broadcast over that image's queries
  * instead of being expanded.  Reductions over queries and samples run in a fixed order (no float atomics).
  *
- * mask_attn: w [B][Q][heads][HW] = softmax over HW of scale * q . k, -inf where pad (MHAttentionMap, head width 32).
- *   q [B][Q][heads*32], k [B][HW][heads*32] token-major, pad [B][HW] bool or NULL.  q, k (and dk) must be
- *   16-byte aligned, else TFB200_E_SHAPE.  backward: dq, dk from dw; ds_ws [B][Q][heads][HW] scratch.            */
+ * mask_attn: w [B][Q][heads][HW] = scale * q . k per head, -inf where pad, then one softmax over each query's
+ *   heads * HW entries together (MHAttentionMap, head width 32): the heads of a query share one partition sum.
+ *   q [B][Q][heads*32], k [B][HW][heads*32] token-major, pad [B][HW] bool or NULL; heads <= 256.  q, k (and dk)
+ *   must be 16-byte aligned, else TFB200_E_SHAPE.  backward: dq, dk from dw; ds_ws [B][Q][heads][HW] scratch.     */
 int tfb200_mask_attn_fwd_f32(const float* q, const float* k, const uint8_t* pad, float* w, int B, int Q, int HW,
                              int heads, float scale, void* stream);
 int tfb200_mask_attn_bwd_f32(const float* q, const float* k, const float* w, const float* dw, float* ds_ws, float* dq,

@@ -39,7 +39,9 @@ def _rand(g, *shape, dev):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-def test_mask_attention_fwd_bwd_with_padding(dev):
+def test_mask_attention_joint_softmax_fwd_bwd_with_padding(dev):
+    """One softmax over each query's heads x positions (MHAttentionMap, detr_segmentation.py:214), padded positions
+    at zero, and dq / dk, against fp64 torch."""
     from trackformer_b200.segmentation import mask_attention
     g = torch.Generator().manual_seed(0)
     B, Q, heads, H, W = 2, 7, 8, 13, 21
@@ -58,7 +60,7 @@ def test_mask_attention_fwd_bwd_with_padding(dev):
     qr, kr = q64.clone().requires_grad_(), k64.clone().requires_grad_()
     logits = torch.einsum("bqnc,bpnc->bqnp", qr.view(B, Q, heads, 32) * scale, kr.view(B, H * W, heads, 32))
     logits = logits.masked_fill(pad[:, None, None, :], float("-inf"))
-    wr = logits.softmax(-1)
+    wr = logits.flatten(2).softmax(-1).view_as(logits)     # one softmax over heads x positions (MHAttentionMap)
     (wr * gout).sum().backward()
     _close(w, wr)
     assert (w[0, :, :, pad[0]] == 0).all()

@@ -92,6 +92,36 @@ def test_cpu_forward_shapes_and_prev_features(oracle_op):
     assert torch.isfinite(out2["pred_masks"]).all()
 
 
+def test_mhattention_map_matches_reference_fixture():
+    """Our MHAttentionMap on the CPU in fp64 against the reference's own module recorded by
+    tests/golden/make_golden_mhattn.py: one softmax over heads x pixels per query, padded pixels at zero, and the
+    gradients of q, k and the four linear parameters."""
+    from conftest import load_golden
+    from trackformer_b200.segmentation import MHAttentionMap
+    z = {k: torch.from_numpy(v) for k, v in load_golden("map", prefix="mhattn_").items()}
+    heads = z["grad_out"].shape[2]
+    attn = MHAttentionMap(z["q"].shape[-1], z["q_weight"].shape[0], heads).double()
+    with torch.no_grad():
+        for m in "qk":
+            getattr(attn, f"{m}_linear").weight.copy_(z[f"{m}_weight"])
+            getattr(attn, f"{m}_linear").bias.copy_(z[f"{m}_bias"])
+    q, k = z["q"].clone().requires_grad_(), z["k"].clone().requires_grad_()
+    w = attn(q, k, z["mask"])
+    (w * z["grad_out"]).sum().backward()
+    torch.testing.assert_close(w, z["weights"], rtol=1e-10, atol=1e-13)
+    torch.testing.assert_close(w.flatten(2).sum(-1), torch.ones(w.shape[:2], dtype=torch.float64))
+    assert (w[1][:, :, z["mask"][1]] == 0).all()
+    head_mass = w.detach().flatten(3).sum(-1)            # the fixture's heads carry very different shares of a row
+    assert float((head_mass.max(-1).values / head_mass.min(-1).values).min()) > 2.0
+    got = {"grad_q": q.grad, "grad_k": k.grad}
+    for m in "qk":
+        got[f"grad_{m}_weight"] = getattr(attn, f"{m}_linear").weight.grad
+        got[f"grad_{m}_bias"] = getattr(attn, f"{m}_linear").bias.grad
+    for name, g in got.items():
+        ref = z[name]
+        torch.testing.assert_close(g, ref, rtol=1e-9, atol=1e-12 * float(ref.abs().max()), msg=name)
+
+
 def _targets_with_masks(seed, sizes, n_boxes):
     g = torch.Generator().manual_seed(seed)
     out = mf.make_targets(seed, len(sizes), 0)
@@ -177,6 +207,7 @@ def test_mask_head_entry_points_validate_arguments():
     odd = ctypes.c_void_p(ctypes.addressof(buf) + 4)
     assert attn(odd, p, None, p, 1, 1, 4, 8, 1.0, None) == -2            # q not 16-byte aligned
     assert attn(p, odd, None, p, 1, 1, 4, 8, 1.0, None) == -2            # k not 16-byte aligned
+    assert attn(p, p, None, p, 1, 1, 4, 257, 1.0, None) == -2            # a q row beyond the shared-memory stage
     attn_bwd = lib.tfb200_mask_attn_bwd_f32
     attn_bwd.argtypes = [vp] * 7 + [i, i, i, i, f, vp]
     assert attn_bwd(p, p, p, p, p, p, odd, 1, 1, 4, 8, 1.0, None) == -2  # dk not 16-byte aligned

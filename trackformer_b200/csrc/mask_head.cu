@@ -60,47 +60,56 @@ __device__ float block_max(float v, float* red) {
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// MHAttentionMap core: w[b][q][h][:] = softmax_p(scale * q[b][q][h] . k[b][p][h], -inf where pad[b][p])
-// one CTA per (b, q, h)
-__global__ void __launch_bounds__(256)
+// MHAttentionMap core: w[b][q] = softmax over (h, p) of scale * q[b][q][h] . k[b][p][h], -inf where pad[b][p].
+// One softmax over all heads and pixels together, as the reference's F.softmax(weights.flatten(2), dim=-1)
+// (detr_segmentation.py:214): the heads of a query share one partition sum.  One CTA per (b, q); its q row
+// (heads * 32 floats) is staged in dynamic shared memory.
+constexpr int kAttnFwdThreads = 512;
+
+__global__ void __launch_bounds__(kAttnFwdThreads)
 mask_attn_fwd_kernel(const float* __restrict__ q, const float* __restrict__ k, const uint8_t* __restrict__ pad,
                      float* __restrict__ w, int Q, int HW, int heads, float scale) {
-  __shared__ float4 qs[kHeadDim / 4];
+  extern __shared__ float4 qs[];                    // [heads][kHeadDim / 4]
   __shared__ float red[32];
-  const int row = blockIdx.x;                       // (b * Q + q) * heads + h
-  const int h = row % heads, bq = row / heads, b = bq / Q;
+  const int bq = blockIdx.x, b = bq / Q;
   const int D = heads * kHeadDim;
-  if (threadIdx.x < kHeadDim / 4)
-    qs[threadIdx.x] = reinterpret_cast<const float4*>(q + int64_t(bq) * D + h * kHeadDim)[threadIdx.x];
+  for (int i = threadIdx.x; i < D / 4; i += blockDim.x)
+    qs[i] = reinterpret_cast<const float4*>(q + int64_t(bq) * D)[i];
   __syncthreads();
-  float* out = w + int64_t(row) * HW;
-  const float* kb = k + int64_t(b) * HW * D + h * kHeadDim;
+  const int64_t n = int64_t(heads) * HW;
+  float* out = w + int64_t(bq) * n;                 // [heads][HW]
+  const float* kb = k + int64_t(b) * HW * D;
+  const uint8_t* pb = pad != nullptr ? pad + int64_t(b) * HW : nullptr;
   float m = -INFINITY;
-  for (int p = threadIdx.x; p < HW; p += blockDim.x) {
-    const float4* kp = reinterpret_cast<const float4*>(kb + int64_t(p) * D);
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) {
+    const int h = int(e / HW), p = int(e % HW);
+    const float4* kp = reinterpret_cast<const float4*>(kb + int64_t(p) * D + h * kHeadDim);
+    const float4* qh = qs + h * (kHeadDim / 4);
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < kHeadDim / 4; ++i) {
-      const float4 a = qs[i], c = kp[i];
+      const float4 a = qh[i], c = kp[i];
       s = fmaf(a.x, c.x, s); s = fmaf(a.y, c.y, s); s = fmaf(a.z, c.z, s); s = fmaf(a.w, c.w, s);
     }
     s *= scale;
-    if (pad != nullptr && pad[int64_t(b) * HW + p]) s = -INFINITY;
-    out[p] = s;
+    if (pb != nullptr && pb[p]) s = -INFINITY;
+    out[e] = s;
     m = fmaxf(m, s);
   }
   m = block_max(m, red);
   float sum = 0.f;
-  for (int p = threadIdx.x; p < HW; p += blockDim.x) {
-    const float e = expf(out[p] - m);
-    out[p] = e;
-    sum += e;
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) {
+    const float x = expf(out[e] - m);
+    out[e] = x;
+    sum += x;
   }
   sum = block_sum(sum, red);
-  for (int p = threadIdx.x; p < HW; p += blockDim.x) out[p] = out[p] / sum;
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) out[e] = out[e] / sum;
 }
 
-// ds = w * (dw - sum(dw * w)) (softmax backward), dq = scale * ds . k; one CTA per (b, q, h)
+// ds = w * (dw - sum(dw * w)) (softmax backward; the sum runs over the whole (b, q) row, all heads and pixels, as the
+// forward's softmax does), dq = scale * ds . k.  One CTA per (b, q, h): each of a row's CTAs computes the row sum
+// itself, in the same order, so they all use the same value.
 __global__ void __launch_bounds__(256)
 mask_attn_bwd_dq_kernel(const float* __restrict__ k, const float* __restrict__ w, const float* __restrict__ dw,
                         float* __restrict__ ds, float* __restrict__ dq, int Q, int HW, int heads, float scale) {
@@ -109,12 +118,15 @@ mask_attn_bwd_dq_kernel(const float* __restrict__ k, const float* __restrict__ w
   const int row = blockIdx.x;
   const int h = row % heads, bq = row / heads, b = bq / Q;
   const int D = heads * kHeadDim;
-  const float* wr = w + int64_t(row) * HW;
-  const float* dwr = dw + int64_t(row) * HW;
-  float* dsr = ds + int64_t(row) * HW;
+  const int64_t n = int64_t(heads) * HW;
+  const float* wq = w + int64_t(bq) * n;
+  const float* dwq = dw + int64_t(bq) * n;
   float dot = 0.f;
-  for (int p = threadIdx.x; p < HW; p += blockDim.x) dot = fmaf(wr[p], dwr[p], dot);
+  for (int64_t e = threadIdx.x; e < n; e += blockDim.x) dot = fmaf(wq[e], dwq[e], dot);
   dot = block_sum(dot, red);
+  const float* wr = wq + int64_t(h) * HW;
+  const float* dwr = dwq + int64_t(h) * HW;
+  float* dsr = ds + int64_t(row) * HW;
   float acc[kHeadDim];
 #pragma unroll
   for (int c = 0; c < kHeadDim; ++c) acc[c] = 0.f;
@@ -493,15 +505,20 @@ inline unsigned blocks_for(int64_t n, int t) { return unsigned((n + t - 1) / t);
 // the attention kernels move q / k rows and dk rows as float4
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// the attention forward stages a query's q row in shared memory: heads * 32 floats, at most 32 KiB
+constexpr int kMaxAttnHeads = 256;
+
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------------------------
 extern "C" int tfb200_mask_attn_fwd_f32(const float* q, const float* k, const uint8_t* pad, float* w, int B, int Q,
                                         int HW, int heads, float scale, void* stream) {
   if (!q || !k || !w) return TFB200_E_NULLPTR;
-  if (B < 0 || Q < 0 || HW <= 0 || heads <= 0 || !aligned16(q) || !aligned16(k)) return TFB200_E_SHAPE;
-  if (int64_t(B) * Q * heads == 0) return 0;
-  mask_attn_fwd_kernel<<<unsigned(B * Q * heads), 256, 0, cudaStream_t(stream)>>>(q, k, pad, w, Q, HW, heads, scale);
+  if (B < 0 || Q < 0 || HW <= 0 || heads <= 0 || heads > kMaxAttnHeads || !aligned16(q) || !aligned16(k))
+    return TFB200_E_SHAPE;
+  if (int64_t(B) * Q == 0) return 0;
+  mask_attn_fwd_kernel<<<unsigned(B * Q), kAttnFwdThreads, sizeof(float) * heads * kHeadDim, cudaStream_t(stream)>>>(
+      q, k, pad, w, Q, HW, heads, scale);
   msda_b200_count_launches(1);
   return int(cudaGetLastError());
 }

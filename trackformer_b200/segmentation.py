@@ -94,7 +94,9 @@ def upsample_add(x: Tensor, a: Tensor) -> Tensor:
 
 
 def mask_attention(q: Tensor, k: Tensor, pad: Optional[Tensor], heads: int, scale: float) -> Tensor:
-    """softmax over positions of ``scale * q . k`` per head: q [B, Q, D], k [B, HW, D] -> [B, Q, heads, HW]."""
+    """``scale * q . k`` per head, -inf where ``pad``, softmax over each query's heads and positions together (one
+    partition sum per query, as MHAttentionMap's ``softmax(weights.flatten(2))``): q [B, Q, D], k [B, HW, D] ->
+    [B, Q, heads, HW]."""
     return _MaskAttn.apply(q, k, pad, heads, scale)
 
 
