@@ -90,6 +90,10 @@ int tfb200_lsa_f32(const float* cost, const int* offsets_dev, int64_t* src, int6
  * optionally, labels [N][Q] int64.  Ties between classes resolve to the smallest index (torch.max).                 */
 int tfb200_detect_postprocess_f32(const float* logits, const float* boxes, const int64_t* sizes_hw, float* packed,
                                   int64_t* labels, int N, int Q, int C, void* stream);
+/* The same rows for the softmax classifier of vanilla DETR (PostProcess, detr.py:446-490): logits [N][Q][C] with the
+ * last column "no object" (C >= 2); score = softmax probability of the best of the first C - 1 classes.            */
+int tfb200_detect_postprocess_softmax_f32(const float* logits, const float* boxes, const int64_t* sizes_hw,
+                                          float* packed, int64_t* labels, int N, int Q, int C, void* stream);
 
 /* clip_grad_norm_ + AdamW (decoupled weight decay) over one contiguous fp32 range of n parameters in one pass
  * (engine.py:147-151 + torch.optim.AdamW of train.py:118).  grad_norm_dev: device scalar holding the global gradient
@@ -189,6 +193,27 @@ int tfb200_small_attn_fwd_f32(const float* q, const float* k, const float* v, co
 int tfb200_small_attn_bwd_f32(const float* q, const float* k, const float* v, const uint8_t* key_pad,
                               const int64_t* seed_dev, const float* out, const float* lse, const float* dout,
                               float* dq, float* dk, float* dv, float* delta_ws, int B, int H, int L,
+                              const int64_t* strides16, float scale, float keep_prob, void* stream);
+
+/* Dense multi-head attention over long key sequences, 32 channels per head (csrc/dense_attn.cu; replaces the core of the
+ * three nn.MultiheadAttention calls of the vanilla transformer, reference models/transformer.py: encoder
+ * self-attention, decoder self- and cross-attention).  Flash-style tiles, both products on tensor cores as split-TF32
+ * (fp32-level accuracy), online softmax in fp32.  q / out / dout / dq are [Lq][B][H][32] VIEWS, k / v / dk / dv
+ * [Lk][B][H][32] VIEWS: channel stride 1, head stride 32, 16-byte aligned base, sequence / batch strides (in elements,
+ * multiples of 4) in
+ *   strides8  = {q_l, q_b, k_l, k_b, v_l, v_b, out_l, out_b}
+ *   strides16 = strides8 + {dout_l, dout_b, dq_l, dq_b, dk_l, dk_b, dv_l, dv_b}
+ * out = dropout(softmax(scale * q k^T + mask)) v; Lq, Lk >= 1 independent; key_pad [B][Lk] (nonzero = ignore that key,
+ * any pattern) or NULL; a query whose keys are all ignored gets a zero output.  seed_dev NULL = no dropout, else
+ * keep_prob in (0, 1] with the mask-free hash RNG keyed by the element index ((b*H + h)*Lq + q)*Lk + k; lse [B][H][Lq]
+ * (saved for the backward); delta_ws [B][H][Lq] scratch.  B*H <= 65535.  The backward uses no atomics: bitwise
+ * reproducible.                                                                                                      */
+int tfb200_dense_attn_fwd_f32(const float* q, const float* k, const float* v, const uint8_t* key_pad,
+                              const int64_t* seed_dev, float* out, float* lse, int B, int H, int Lq, int Lk,
+                              const int64_t* strides8, float scale, float keep_prob, void* stream);
+int tfb200_dense_attn_bwd_f32(const float* q, const float* k, const float* v, const uint8_t* key_pad,
+                              const int64_t* seed_dev, const float* out, const float* lse, const float* dout,
+                              float* dq, float* dk, float* dv, float* delta_ws, int B, int H, int Lq, int Lk,
                               const int64_t* strides16, float scale, float keep_prob, void* stream);
 
 /* One frame of the online tracker's bookkeeping on the device (csrc/track_step.cu; reference models/tracker.py:266-548:

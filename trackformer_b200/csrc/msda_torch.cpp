@@ -471,6 +471,75 @@ std::vector<at::Tensor> small_attention_backward(const at::Tensor& q, const at::
   return {dq, dk, dv};
 }
 
+// Dense attention over long key sequences (csrc/dense_attn.cu): q [Lq, B, H, 32], k / v [Lk, B, H, 32] views (channel
+// stride 1, head stride 32); key_pad [B, Lk] bool or None; seed None = no dropout.  Returns {out [Lq, B, H, 32],
+// lse [B, H, Lq]}.
+static const uint8_t* dense_key_pad(const c10::optional<at::Tensor>& key_pad, at::Tensor& kpc, int64_t B, int64_t Lk,
+                                    const at::Tensor& q) {
+  if (!key_pad.has_value() || !key_pad->defined()) return nullptr;
+  kpc = key_pad->contiguous();
+  TORCH_CHECK(kpc.device() == q.device() && kpc.dim() == 2 && kpc.size(0) == B && kpc.size(1) == Lk &&
+                  kpc.element_size() == 1,
+              "dense_attention: key_pad must be a bool [B, Lk] tensor on the device of q");
+  return static_cast<const uint8_t*>(kpc.data_ptr());
+}
+static void check_dense_shapes(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v) {
+  check_view(q, "q"); check_view(k, "k"); check_view(v, "v");
+  TORCH_CHECK(k.device() == q.device() && v.device() == q.device() && k.sizes() == v.sizes() && k.size(1) == q.size(1) &&
+                  k.size(2) == q.size(2),
+              "dense_attention: q [Lq, B, H, 32] and k, v [Lk, B, H, 32] must agree on B and H");
+}
+
+std::vector<at::Tensor> dense_attention_forward(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v,
+                                                const c10::optional<at::Tensor>& key_pad,
+                                                const c10::optional<at::Tensor>& seed, double scale, double keep_prob) {
+  check_dense_shapes(q, k, v);
+  const int64_t Lq = q.size(0), B = q.size(1), H = q.size(2), Lk = k.size(0);
+  const c10::cuda::CUDAGuard guard(q.device());
+  at::Tensor out = at::empty({Lq, B, H, 32}, q.options());
+  at::Tensor lse = at::empty({B, H, Lq}, q.options());
+  at::Tensor kpc;
+  const uint8_t* kp = dense_key_pad(key_pad, kpc, B, Lk, q);
+  const int64_t* sp = (seed.has_value() && seed->defined()) ? seed->data_ptr<int64_t>() : nullptr;
+  const int64_t st[8] = {q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1), out.stride(0), out.stride(1)};
+  const int rc = tfb200_dense_attn_fwd_f32(q.data_ptr<float>(), k.data_ptr<float>(), v.data_ptr<float>(), kp, sp,
+                                           out.data_ptr<float>(), lse.data_ptr<float>(), int(B), int(H), int(Lq), int(Lk),
+                                           st, float(scale), float(keep_prob), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "dense_attention_forward failed (code ", rc, ")");
+  return {out, lse};
+}
+
+std::vector<at::Tensor> dense_attention_backward(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v,
+                                                 const c10::optional<at::Tensor>& key_pad,
+                                                 const c10::optional<at::Tensor>& seed, const at::Tensor& out,
+                                                 const at::Tensor& lse, const at::Tensor& grad_out, double scale,
+                                                 double keep_prob) {
+  check_dense_shapes(q, k, v);
+  check_view(out, "out");
+  const at::Tensor go = grad_out.contiguous();
+  check_view(go, "grad_out");
+  const int64_t Lq = q.size(0), B = q.size(1), H = q.size(2), Lk = k.size(0);
+  TORCH_CHECK(out.sizes() == q.sizes() && go.sizes() == q.sizes() && lse.is_contiguous() && lse.numel() == B * H * Lq,
+              "dense_attention_backward: out / grad_out must be [Lq, B, H, 32] and lse [B, H, Lq]");
+  const c10::cuda::CUDAGuard guard(q.device());
+  at::Tensor dq = at::empty({Lq, B, H, 32}, q.options()), dk = at::empty({Lk, B, H, 32}, q.options()),
+             dv = at::empty({Lk, B, H, 32}, q.options());
+  at::Tensor delta = at::empty({B, H, Lq}, q.options());
+  at::Tensor kpc;
+  const uint8_t* kp = dense_key_pad(key_pad, kpc, B, Lk, q);
+  const int64_t* sp = (seed.has_value() && seed->defined()) ? seed->data_ptr<int64_t>() : nullptr;
+  const int64_t st[16] = {q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1), out.stride(0),
+                          out.stride(1), go.stride(0), go.stride(1), dq.stride(0), dq.stride(1), dk.stride(0), dk.stride(1),
+                          dv.stride(0), dv.stride(1)};
+  const int rc = tfb200_dense_attn_bwd_f32(q.data_ptr<float>(), k.data_ptr<float>(), v.data_ptr<float>(), kp, sp,
+                                           out.data_ptr<float>(), lse.data_ptr<float>(), go.data_ptr<float>(),
+                                           dq.data_ptr<float>(), dk.data_ptr<float>(), dv.data_ptr<float>(),
+                                           delta.data_ptr<float>(), int(B), int(H), int(Lq), int(Lk), st, float(scale),
+                                           float(keep_prob), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "dense_attention_backward failed (code ", rc, ")");
+  return {dq, dk, dv};
+}
+
 // boxes = sigmoid(delta + inverse_sigmoid(ref)) (csrc/box_refine.cu); delta [..., 4], ref [..., 2 or 4]
 at::Tensor refine_boxes_forward(const at::Tensor& delta, const at::Tensor& ref, double eps) {
   TORCH_CHECK(delta.is_cuda() && ref.is_cuda() && delta.scalar_type() == at::kFloat && ref.scalar_type() == at::kFloat &&
@@ -693,7 +762,8 @@ std::vector<at::Tensor> set_loss_backward(const at::Tensor& unit_logits, const a
 }
 
 // ---- detection post-processing for the tracker (deformable_detr.py:286-334) ------------------------------------------
-std::vector<at::Tensor> detect_postprocess(const at::Tensor& logits, const at::Tensor& boxes, const at::Tensor& sizes_hw) {
+std::vector<at::Tensor> detect_postprocess(const at::Tensor& logits, const at::Tensor& boxes, const at::Tensor& sizes_hw,
+                                           bool softmax) {
   TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.dim() == 3, "detect_postprocess: logits must be [N,Q,C] fp32 CUDA");
   TORCH_CHECK(boxes.is_cuda() && boxes.scalar_type() == at::kFloat && boxes.dim() == 3 && boxes.size(2) == 4, "detect_postprocess: boxes must be [N,Q,4] fp32 CUDA");
   TORCH_CHECK(sizes_hw.is_cuda() && sizes_hw.scalar_type() == at::kLong && sizes_hw.dim() == 2 && sizes_hw.size(1) == 2, "detect_postprocess: sizes must be [N,2] int64 CUDA");
@@ -703,9 +773,9 @@ std::vector<at::Tensor> detect_postprocess(const at::Tensor& logits, const at::T
   auto lg = logits.contiguous(), bx = boxes.contiguous(), sz = sizes_hw.contiguous();
   auto packed = at::empty({N, Q, 6}, lg.options());
   auto labels = at::empty({N, Q}, lg.options().dtype(at::kLong));
-  const int rc = tfb200_detect_postprocess_f32(lg.data_ptr<float>(), bx.data_ptr<float>(), sz.data_ptr<int64_t>(),
-                                               packed.data_ptr<float>(), labels.data_ptr<int64_t>(), int(N), int(Q), int(C),
-                                               at::cuda::getCurrentCUDAStream().stream());
+  const int rc = (softmax ? tfb200_detect_postprocess_softmax_f32 : tfb200_detect_postprocess_f32)(
+      lg.data_ptr<float>(), bx.data_ptr<float>(), sz.data_ptr<int64_t>(), packed.data_ptr<float>(),
+      labels.data_ptr<int64_t>(), int(N), int(Q), int(C), at::cuda::getCurrentCUDAStream().stream());
   TORCH_CHECK(rc == 0, "detect_postprocess failed (code ", rc, ")");
   return {packed, labels};
 }
@@ -1095,6 +1165,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("sampling_prep_backward", &sampling_prep_backward);
   m.def("small_attention_forward", &small_attention_forward);
   m.def("small_attention_backward", &small_attention_backward);
+  m.def("dense_attention_forward", &dense_attention_forward);
+  m.def("dense_attention_backward", &dense_attention_backward);
   m.def("refine_boxes_forward", &refine_boxes_forward);
   m.def("refine_boxes_backward", &refine_boxes_backward);
   m.def("tf32_linear", &tf32_linear);
@@ -1103,7 +1175,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("tf32_linear_wgrad", &tf32_linear_wgrad);
   m.def("relu_dropout_forward", &relu_dropout_forward);
   m.def("relu_dropout_backward", &relu_dropout_backward);
-  m.def("detect_postprocess", &detect_postprocess);
+  m.def("detect_postprocess", &detect_postprocess, pybind11::arg("logits"), pybind11::arg("boxes"),
+        pybind11::arg("sizes_hw"), pybind11::arg("softmax") = false);
   m.def("flat_adamw", &flat_adamw);
   m.def("frozen_bn_act_forward", &frozen_bn_act_forward);
   m.def("frozen_bn_act_backward", &frozen_bn_act_backward);

@@ -9,6 +9,7 @@
 //   labels[n][q] = label as int64 (for the reference-shaped result dict)
 // One warp per query: lanes stride the class axis, the arg-max keeps the FIRST maximal class like torch.max.
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
@@ -16,6 +17,9 @@
 
 namespace {
 
+// kSoftmax = false: sigmoid scores over all C classes (DeformablePostProcess, focal loss);
+// kSoftmax = true:  softmax over the C logits (the last one is "no object"), best of the first C - 1 (PostProcess)
+template <bool kSoftmax>
 __global__ void __launch_bounds__(256)
 detect_postprocess_kernel(const float* __restrict__ logits, const float* __restrict__ boxes,
                           const int64_t* __restrict__ sizes, float* __restrict__ packed, int64_t* __restrict__ labels,
@@ -24,11 +28,27 @@ detect_postprocess_kernel(const float* __restrict__ logits, const float* __restr
   const int64_t row = int64_t(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= int64_t(N) * Q) return;
   const float* lg = logits + row * C;
-  float best = -1.f;          // sigmoid scores are >= 0
+  float best = -1.f;          // sigmoid / softmax scores are >= 0
   int arg = 0x7fffffff;
-  for (int c = lane; c < C; c += 32) {
-    const float s = 1.f / (1.f + expf(-__ldg(lg + c)));
-    if (s > best) { best = s; arg = c; }     // strict: the smallest class index wins inside a lane
+  if (kSoftmax) {
+    float mx = -INFINITY;
+    for (int c = lane; c < C; c += 32) mx = fmaxf(mx, __ldg(lg + c));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    float sum = 0.f;
+    for (int c = lane; c < C; c += 32) sum += expf(__ldg(lg + c) - mx);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    const float inv = 1.f / sum;
+    for (int c = lane; c < C - 1; c += 32) {
+      const float s = expf(__ldg(lg + c) - mx) * inv;
+      if (s > best) { best = s; arg = c; }
+    }
+  } else {
+    for (int c = lane; c < C; c += 32) {
+      const float s = 1.f / (1.f + expf(-__ldg(lg + c)));
+      if (s > best) { best = s; arg = c; }     // strict: the smallest class index wins inside a lane
+    }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
@@ -60,7 +80,19 @@ extern "C" int tfb200_detect_postprocess_f32(const float* logits, const float* b
   if (N == 0 || Q == 0) return 0;
   const int64_t rows = int64_t(N) * Q;
   const int grid = int((rows + 7) / 8);
-  detect_postprocess_kernel<<<grid, 256, 0, cudaStream_t(stream)>>>(logits, boxes, sizes_hw, packed, labels, N, Q, C);
+  detect_postprocess_kernel<false><<<grid, 256, 0, cudaStream_t(stream)>>>(logits, boxes, sizes_hw, packed, labels, N, Q, C);
+  msda_b200_count_launches(1);
+  return int(cudaGetLastError());
+}
+
+extern "C" int tfb200_detect_postprocess_softmax_f32(const float* logits, const float* boxes, const int64_t* sizes_hw,
+                                                     float* packed, int64_t* labels, int N, int Q, int C, void* stream) {
+  if (!logits || !boxes || !sizes_hw || !packed) return TFB200_E_NULLPTR;
+  if (N < 0 || Q < 0 || C < 2) return TFB200_E_SHAPE;
+  if (N == 0 || Q == 0) return 0;
+  const int64_t rows = int64_t(N) * Q;
+  const int grid = int((rows + 7) / 8);
+  detect_postprocess_kernel<true><<<grid, 256, 0, cudaStream_t(stream)>>>(logits, boxes, sizes_hw, packed, labels, N, Q, C);
   msda_b200_count_launches(1);
   return int(cudaGetLastError());
 }

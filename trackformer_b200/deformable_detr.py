@@ -1,6 +1,7 @@
-"""Deformable-DETR detector shell around the H100 transformer.
+"""DETR and Deformable-DETR detectors around the H100 transformers.
 
-Mirror of ``DETR`` (constructor state only: src/trackformer/models/detr.py:17-54), ``MLP`` (:493-507) and
+Mirror of ``DETR`` (src/trackformer/models/detr.py:17-128, the vanilla detector on transformer.py), ``PostProcess``
+(:446-490), ``MLP`` (:493-507) and
 ``DeformableDETR`` (src/trackformer/models/deformable_detr.py:29-283) with the same forward signature
 ``(samples, targets=None, prev_features=None) -> (out, targets, features_all, memory_per_level, hs)`` and the
 same parameter names (``input_proj.{l}.{0,1}``, ``class_embed.{k}``, ``bbox_embed.{k}.layers.{j}``,
@@ -70,6 +71,37 @@ class DETR(nn.Module):
     @torch.jit.unused
     def _set_aux_loss(self, outputs_class, outputs_coord):
         return [{"pred_logits": a, "pred_boxes": b} for a, b in zip(outputs_class[:-1], outputs_coord[:-1])]
+
+    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None):
+        """Vanilla DETR (detr.py:62-128): single-level ``input_proj``, track queries as zero ``query_embed`` rows whose
+        decoder input is ``track_query_hs_embeds``.  ``prev_features`` is accepted (the tracker passes it) and ignored:
+        vanilla DETR has no multi-frame path.  ``track_query_padding`` [K] per image marks filler track queries, hidden
+        from the others as self-attention keys (GraphedDetector, TrainStep).  Unlike the reference, the targets'
+        ``track_query_hs_embeds`` are not overwritten with the full decoder input rows."""
+        if not isinstance(samples, NestedTensor):
+            samples = nested_tensor_from_tensor_list(samples)
+        features, pos = self.backbone(samples)
+        src, mask = features[-1].decompose()
+        assert mask is not None
+        src = self.input_proj(src)
+        bs = src.shape[0]
+        query_embed = self.query_embed.weight.unsqueeze(1).repeat(1, bs, 1)
+        tgt = tgt_pad = None
+        if targets is not None and "track_query_hs_embeds" in targets[0]:
+            track_hs = torch.stack([t["track_query_hs_embeds"] for t in targets]).transpose(0, 1)    # [K, B, C]
+            query_embed = torch.cat([torch.zeros_like(track_hs), query_embed])
+            tgt = torch.cat([track_hs, torch.zeros_like(query_embed[track_hs.shape[0]:])])
+            if "track_query_padding" in targets[0]:
+                filler = torch.stack([t["track_query_padding"] for t in targets])
+                tgt_pad = torch.cat([filler, filler.new_zeros(bs, self.num_queries)], 1)
+        hs, hs_without_norm, memory = self.transformer(src, mask, query_embed, pos[-1], tgt,
+                                                       tgt_key_padding_mask=tgt_pad)
+        outputs_class = self.class_embed(hs)
+        outputs_coord = self.bbox_embed(hs).sigmoid()
+        out = {"pred_logits": outputs_class[-1], "pred_boxes": outputs_coord[-1], "hs_embed": hs_without_norm[-1]}
+        if self.aux_loss:
+            out["aux_outputs"] = self._set_aux_loss(outputs_class, outputs_coord)
+        return out, targets, features, memory, hs
 
 
 class _CallScratch:
@@ -226,6 +258,44 @@ class DeformableDETR(DETR):
             per_level.append(memory[:, ofs:ofs + h * w].permute(0, 2, 1).view(bsz, ch, h, w))
             ofs += h * w
         return out, targets, features_all, per_level, hs
+
+
+class PostProcess(nn.Module):
+    """Softmax scores over the C + 1 classes, best real class per query, ``scores_no_object``, boxes scaled to the
+    target sizes (detr.py:446-490).  ``packed()`` gives the [N, Q, 6] rows of ``DeformablePostProcess.packed`` --
+    on CUDA one launch of the softmax twin of the fused kernel (csrc/track_post.cu) -- so the trackers take their
+    one-copy route unchanged."""
+
+    @torch.no_grad()
+    def packed(self, outputs, target_sizes):
+        logits, boxes = outputs["pred_logits"], outputs["pred_boxes"]
+        assert len(logits) == len(target_sizes) and target_sizes.shape[1] == 2
+        if logits.is_cuda and logits.dtype == torch.float32:
+            from .ext import load
+            rows, labels = load().detect_postprocess(logits, boxes, target_sizes.to(logits.device, torch.int64), True)
+            rows._labels = labels
+            return rows
+        scores, labels = F.softmax(logits, -1)[..., :-1].max(-1)
+        img_h, img_w = target_sizes.unbind(1)
+        xyxy = box_cxcywh_to_xyxy(boxes) * torch.stack([img_w, img_h, img_w, img_h], dim=1)[:, None, :]
+        rows = torch.cat([scores[..., None], labels[..., None].to(scores.dtype), xyxy.to(scores.dtype)], -1)
+        rows._labels = labels
+        return rows
+
+    @torch.no_grad()
+    def forward(self, outputs, target_sizes, results_mask=None):
+        out_logits, out_bbox = outputs["pred_logits"], outputs["pred_boxes"]
+        assert len(out_logits) == len(target_sizes) and target_sizes.shape[1] == 2
+        prob = F.softmax(out_logits, -1)
+        scores, labels = prob[..., :-1].max(-1)
+        img_h, img_w = target_sizes.unbind(1)
+        boxes = box_cxcywh_to_xyxy(out_bbox) * torch.stack([img_w, img_h, img_w, img_h], dim=1)[:, None, :]
+        results = [{"scores": s, "labels": l, "boxes": b, "scores_no_object": n}
+                   for s, l, b, n in zip(scores, labels, boxes, prob[..., -1])]
+        if results_mask is not None:
+            for i, keep in enumerate(results_mask):
+                results[i] = {k: v[keep] for k, v in results[i].items()}
+        return results
 
 
 class DeformablePostProcess(nn.Module):

@@ -24,7 +24,7 @@ from contextlib import nullcontext
 import torch
 from torch import nn
 
-from .deformable_detr import DeformableDETR
+from .deformable_detr import DETR, DeformableDETR
 from .matcher import HungarianMatcher
 from .util import NestedTensor
 
@@ -143,4 +143,10 @@ class DETRTrackingBase(nn.Module):
 class DeformableDETRTracking(DETRTrackingBase, DeformableDETR):
     def __init__(self, tracking_kwargs, detr_kwargs):
         DeformableDETR.__init__(self, **detr_kwargs)
+        DETRTrackingBase.__init__(self, **tracking_kwargs)
+
+
+class DETRTracking(DETRTrackingBase, DETR):
+    def __init__(self, tracking_kwargs, detr_kwargs):
+        DETR.__init__(self, **detr_kwargs)
         DETRTrackingBase.__init__(self, **tracking_kwargs)

@@ -1,13 +1,15 @@
 """Model factory + the reference's hyper-parameter sets for the hot path.
 
-``build_model(args)`` mirrors src/trackformer/models/__init__.py:16-130 for the deformable, box-only
-configurations (detection and tracking): it returns ``(model, criterion, postprocessors)`` with the same class
-counts (:17-26), loss weights (:83-99) and focal-loss post-processor (:117-118).
+``build_model(args)`` mirrors src/trackformer/models/__init__.py:16-130: it returns ``(model, criterion,
+postprocessors)`` with the same class counts (:17-26), model classes (:48-83: ``DeformableDETR[Tracking]`` or, with
+``deformable=False``, the vanilla ``DETR[Tracking]``), loss weights (:83-99) and post-processor (:120-123: sigmoid
+``DeformablePostProcess`` with the focal loss, softmax ``PostProcess`` otherwise).
 
 With ``masks=True`` it builds the segmentation models of src/trackformer/models/detr_segmentation.py
-(``DeformableDETRSegm`` / ``DeformableDETRSegmTracking``) and adds the ``masks`` loss and the ``segm``
+(``[Deformable]DETRSegm`` / ``[Deformable]DETRSegmTracking``) and adds the ``masks`` loss and the ``segm``
 post-processor (:42-45, 86-88, 103-104, 121-125); the panoptic post-processor is not provided.
 
+``vanilla_args(...)`` gives cfgs/train.yaml alone (vanilla DETR), optionally with train_tracking.yaml.
 ``default_args(...)`` reproduces the values of cfgs/train.yaml overlaid with train_deformable.yaml and,
 optionally, train_tracking.yaml / train_multi_frame.yaml (the named sacred configs of src/train.py:24-35), so
 the benchmark and the tests can instantiate the exact reference geometry without the YAML files (they do not
@@ -21,11 +23,12 @@ import torch
 
 from .backbone import build_backbone
 from .criterion import SetCriterion
-from .deformable_detr import DeformableDETR, DeformablePostProcess
+from .deformable_detr import DETR, DeformableDETR, DeformablePostProcess, PostProcess
 from .deformable_transformer import build_deforamble_transformer
-from .detr_tracking import DeformableDETRTracking
+from .detr_tracking import DeformableDETRTracking, DETRTracking
 from .matcher import build_matcher
-from .segmentation import DeformableDETRSegm, DeformableDETRSegmTracking, PostProcessSegm
+from .segmentation import DeformableDETRSegm, DeformableDETRSegmTracking, DETRSegm, DETRSegmTracking, PostProcessSegm
+from .transformer import build_transformer
 
 _TRAIN_YAML = dict(   # cfgs/train.yaml (model / loss keys only)
     lr=2e-4, lr_backbone_names=["backbone.0"], lr_backbone=2e-5,
@@ -67,6 +70,17 @@ def default_args(tracking: bool = False, multi_frame: bool = False, **overrides)
     return Namespace(**cfg)
 
 
+def vanilla_args(tracking: bool = False, masks: bool = False, **overrides) -> Namespace:
+    """cfgs/train.yaml as it stands (vanilla DETR: ``deformable: false``, 100 queries, softmax classifier) and, with
+    ``tracking``, train_tracking.yaml on top; ``masks`` sets the segmentation head."""
+    cfg = dict(_TRAIN_YAML)
+    if tracking:
+        cfg.update(_TRACKING_YAML)
+    cfg["masks"] = masks
+    cfg.update(overrides)
+    return Namespace(**cfg)
+
+
 def num_classes_for(dataset: str) -> int:
     if dataset == "coco":
         return 91
@@ -78,8 +92,6 @@ def num_classes_for(dataset: str) -> int:
 
 
 def build_model(args):
-    if not args.deformable:
-        raise NotImplementedError("only the deformable path is built (vanilla DETR is outside the hot path)")
     if args.masks and args.dataset == "coco_panoptic":
         raise NotImplementedError("the panoptic post-processor is not provided")
     num_classes = num_classes_for(args.dataset)
@@ -87,24 +99,32 @@ def build_model(args):
     matcher = build_matcher(args)
     detr_kwargs = dict(
         backbone=backbone, num_classes=num_classes - 1 if args.focal_loss else num_classes,
-        num_queries=args.num_queries, aux_loss=args.aux_loss, overflow_boxes=args.overflow_boxes,
-        transformer=build_deforamble_transformer(args), num_feature_levels=args.num_feature_levels,
-        with_box_refine=args.with_box_refine, two_stage=args.two_stage,
-        multi_frame_attention=args.multi_frame_attention, multi_frame_encoding=args.multi_frame_encoding,
-        merge_frame_features=args.merge_frame_features)
-    if args.tracking:
-        tracking_kwargs = dict(
-            track_query_false_positive_prob=args.track_query_false_positive_prob,
-            track_query_false_negative_prob=args.track_query_false_negative_prob,
-            matcher=matcher, backprop_prev_frame=args.track_backprop_prev_frame)
-        if args.masks:
-            model = DeformableDETRSegmTracking({"freeze_detr": args.freeze_detr}, tracking_kwargs, detr_kwargs)
-        else:
-            model = DeformableDETRTracking(tracking_kwargs, detr_kwargs)
-    elif args.masks:
-        model = DeformableDETRSegm({"freeze_detr": args.freeze_detr}, detr_kwargs)
+        num_queries=args.num_queries, aux_loss=args.aux_loss, overflow_boxes=args.overflow_boxes)
+    tracking_kwargs = dict(
+        track_query_false_positive_prob=args.track_query_false_positive_prob,
+        track_query_false_negative_prob=args.track_query_false_negative_prob,
+        matcher=matcher, backprop_prev_frame=args.track_backprop_prev_frame)
+    mask_kwargs = {"freeze_detr": args.freeze_detr}
+    if args.deformable:
+        detr_kwargs.update(
+            transformer=build_deforamble_transformer(args), num_feature_levels=args.num_feature_levels,
+            with_box_refine=args.with_box_refine, two_stage=args.two_stage,
+            multi_frame_attention=args.multi_frame_attention, multi_frame_encoding=args.multi_frame_encoding,
+            merge_frame_features=args.merge_frame_features)
+        classes = (DeformableDETR, DeformableDETRTracking, DeformableDETRSegm, DeformableDETRSegmTracking)
     else:
-        model = DeformableDETR(**detr_kwargs)
+        detr_kwargs["transformer"] = build_transformer(args)
+        classes = (DETR, DETRTracking, DETRSegm, DETRSegmTracking)
+    plain, tracking, segm, segm_tracking = classes
+    if args.tracking:
+        if args.masks:
+            model = segm_tracking(mask_kwargs, tracking_kwargs, detr_kwargs)
+        else:
+            model = tracking(tracking_kwargs, detr_kwargs)
+    elif args.masks:
+        model = segm(mask_kwargs, detr_kwargs)
+    else:
+        model = plain(**detr_kwargs)
 
     weight_dict = {"loss_ce": args.cls_loss_coef, "loss_bbox": args.bbox_loss_coef, "loss_giou": args.giou_loss_coef}
     if args.masks:
@@ -120,7 +140,7 @@ def build_model(args):
         focal_gamma=args.focal_gamma, tracking=args.tracking,
         track_query_false_positive_eos_weight=args.track_query_false_positive_eos_weight)
     criterion.to(torch.device(args.device))
-    postprocessors = {"bbox": DeformablePostProcess()}
+    postprocessors = {"bbox": DeformablePostProcess() if args.focal_loss else PostProcess()}
     if args.masks:
         postprocessors["segm"] = PostProcessSegm()
     return model, criterion, postprocessors

@@ -1,6 +1,6 @@
-"""Segmentation heads of the deformable detector: ``DeformableDETRSegm`` and ``DeformableDETRSegmTracking``.
+"""Segmentation heads: ``DETRSegm``, ``DETRSegmTracking``, ``DeformableDETRSegm`` and ``DeformableDETRSegmTracking``.
 
-Mirror of src/trackformer/models/detr_segmentation.py:29-253 for the deformable classes: same class layout
+Mirror of src/trackformer/models/detr_segmentation.py:29-253: same class layout
 (``DETRSegmBase`` mixed in front of ``DETRTrackingBase`` / ``DeformableDETR``, so the previous-frame forwards of tracking
 training run without the mask head), constructor arguments, ``freeze_detr``, initialisation and parameter names
 (``bbox_attention.{q,k}_linear.*``, ``mask_head.{lay1..5,gn1..5,out_lay,adapter1..3}.*``), and ``pred_masks``
@@ -26,7 +26,7 @@ from torch.autograd import Function
 from torch.autograd.function import once_differentiable
 
 from . import ext
-from .deformable_detr import DeformableDETR
+from .deformable_detr import DETR, DeformableDETR
 from .detr_tracking import DETRTrackingBase
 from .fused_linear import linear as fused_linear
 from .util import NestedTensor
@@ -232,19 +232,38 @@ class DETRSegmBase(nn.Module):
         """Mask logits ``[B, len(rows), H/4, W/4]`` of the query rows ``rows`` (all rows if None) from the outputs of
         ``detect``.  Every query has its own attention softmax and its own GroupNorm sample, so a row's logits do not
         depend on which other rows are computed with it."""
-        src, mask = features[-2].decompose()                     # stride 16 (layer3)
+        if isinstance(memory, list):                               # deformable: per-level memory, stride 16 (layer3)
+            src, mask = features[-2].decompose()
+            src = self.input_proj[-3](src)
+            if mask.shape[-2:] != src.shape[-2:]:
+                mask = F.interpolate(mask[None].float(), size=src.shape[-2:]).to(torch.bool)[0]
+            fpns = [features[-2].tensors, features[-3].tensors, features[-4].tensors]
+            memory = memory[-3]
+        else:                                                      # vanilla DETR: stride-32 memory [B, C, h, w]
+            src, mask = features[-1].decompose()
+            src = self.input_proj(src)
+            fpns = [features[2].tensors, features[1].tensors, features[0].tensors]
         batch_size = src.shape[0]
-        src = self.input_proj[-3](src)
-        if mask.shape[-2:] != src.shape[-2:]:
-            mask = F.interpolate(mask[None].float(), size=src.shape[-2:]).to(torch.bool)[0]
-        fpns = [features[-2].tensors, features[-3].tensors, features[-4].tensors]
 
         q = hs[-1]
         if rows is not None:
             q = q.index_select(1, torch.as_tensor(rows, dtype=torch.long, device=q.device))
-        bbox_mask = self.bbox_attention(q, memory[-3], mask=mask)
+        bbox_mask = self.bbox_attention(q, memory, mask=mask)
         seg_masks = self.mask_head(src, bbox_mask, fpns)
         return seg_masks.view(batch_size, q.shape[1], seg_masks.shape[-2], seg_masks.shape[-1])
+
+
+class DETRSegm(DETRSegmBase, DETR):
+    def __init__(self, mask_kwargs, detr_kwargs):
+        DETR.__init__(self, **detr_kwargs)
+        DETRSegmBase.__init__(self, **mask_kwargs)
+
+
+class DETRSegmTracking(DETRSegmBase, DETRTrackingBase, DETR):
+    def __init__(self, mask_kwargs, tracking_kwargs, detr_kwargs):
+        DETR.__init__(self, **detr_kwargs)
+        DETRTrackingBase.__init__(self, **tracking_kwargs)
+        DETRSegmBase.__init__(self, **mask_kwargs)
 
 
 class DeformableDETRSegm(DETRSegmBase, DeformableDETR):
