@@ -74,6 +74,24 @@ def test_dropout_is_deterministic_and_differentiated_consistently(op, cuda_devic
             assert abs(num - float(t.grad[idx])) < 2e-2 * max(1.0, abs(num)), (idx, num, float(t.grad[idx]))
 
 
+def test_key_padding_of_the_wrong_shape_or_device_is_rejected(op, cuda_device):
+    """A [L, B] (transposed) or flattened mask has the right element count but the wrong layout, and a host mask cannot
+    be read by the kernel: errors in both directions, not a silently wrong pattern."""
+    from trackformer_b200.small_attention import _SmallAttention
+    g = torch.Generator().manual_seed(9)
+    L, B, H = 40, 2, 2
+    q, k, v = (torch.randn(L, B, H, 32, generator=g).to(cuda_device) for _ in range(3))
+    pad = torch.zeros(B, L, dtype=torch.bool, device=cuda_device)
+    pad[1, 30:] = True
+    out, lse = op.small_attention_forward(q, k, v, pad, None, 32 ** -0.5, 1.0)
+    op.small_attention_backward(q, k, v, pad, None, out, lse, out, 32 ** -0.5, 1.0)
+    for bad in (pad.t().contiguous(), pad.flatten(), pad.cpu()):
+        with pytest.raises(RuntimeError, match="key_pad"):
+            _SmallAttention.apply(q, k, v, bad, None, 32 ** -0.5, 1.0)
+        with pytest.raises(RuntimeError, match="key_pad"):
+            op.small_attention_backward(q, k, v, bad, None, out, lse, out, 32 ** -0.5, 1.0)
+
+
 def test_module_replacement_equals_stock_multihead_attention(cuda_device):
     """mha_forward(module, ...) against module(...) itself (eval mode: no dropout), outputs and parameter gradients."""
     from trackformer_b200 import small_attention

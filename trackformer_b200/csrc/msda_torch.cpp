@@ -414,6 +414,17 @@ static void check_view(const at::Tensor& t, const char* name) {
                   t.stride(1) % 4 == 0,
               "small_attention: ", name, " must be an fp32 CUDA [L, B, H, 32] view with 16-byte aligned rows");
 }
+// key_pad [B, L] on the device of q, or nullptr when absent.  Shape, not element count: a transposed [L, B] or flattened
+// mask holds B * L elements too and would be read as a different pattern; a host mask would be dereferenced on the GPU.
+static const uint8_t* checked_key_pad(const c10::optional<at::Tensor>& key_pad, at::Tensor& kpc, int64_t B, int64_t L,
+                                      const at::Tensor& q, const char* op) {
+  if (!key_pad.has_value() || !key_pad->defined()) return nullptr;
+  kpc = key_pad->contiguous();
+  TORCH_CHECK(kpc.device() == q.device() && kpc.dim() == 2 && kpc.size(0) == B && kpc.size(1) == L &&
+                  kpc.element_size() == 1,
+              op, ": key_pad must be a bool [B, Lk] tensor on the device of q");
+  return static_cast<const uint8_t*>(kpc.data_ptr());
+}
 std::vector<at::Tensor> small_attention_forward(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v,
                                                 const c10::optional<at::Tensor>& key_pad,
                                                 const c10::optional<at::Tensor>& seed, double scale, double keep_prob) {
@@ -423,13 +434,8 @@ std::vector<at::Tensor> small_attention_forward(const at::Tensor& q, const at::T
   const c10::cuda::CUDAGuard guard(q.device());
   at::Tensor out = at::empty({L, B, H, 32}, q.options());
   at::Tensor lse = at::empty({B, H, L}, q.options());
-  const uint8_t* kp = nullptr;
   at::Tensor kpc;
-  if (key_pad.has_value() && key_pad->defined()) {
-    kpc = key_pad->contiguous();
-    TORCH_CHECK(kpc.numel() == B * L && kpc.element_size() == 1, "small_attention: key_pad must be a bool [B, L] tensor");
-    kp = static_cast<const uint8_t*>(kpc.data_ptr());
-  }
+  const uint8_t* kp = checked_key_pad(key_pad, kpc, B, L, q, "small_attention");
   const int64_t* sp = (seed.has_value() && seed->defined()) ? seed->data_ptr<int64_t>() : nullptr;
   const int64_t st[8] = {q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1), out.stride(0), out.stride(1)};
   const int rc = tfb200_small_attn_fwd_f32(q.data_ptr<float>(), k.data_ptr<float>(), v.data_ptr<float>(), kp, sp,
@@ -452,12 +458,8 @@ std::vector<at::Tensor> small_attention_backward(const at::Tensor& q, const at::
   at::Tensor dq = at::empty({L, B, H, 32}, q.options()), dk = at::empty({L, B, H, 32}, q.options()),
              dv = at::empty({L, B, H, 32}, q.options());
   at::Tensor delta = at::empty({B, H, L}, q.options());
-  const uint8_t* kp = nullptr;
   at::Tensor kpc;
-  if (key_pad.has_value() && key_pad->defined()) {
-    kpc = key_pad->contiguous();
-    kp = static_cast<const uint8_t*>(kpc.data_ptr());
-  }
+  const uint8_t* kp = checked_key_pad(key_pad, kpc, B, L, q, "small_attention_backward");
   const int64_t* sp = (seed.has_value() && seed->defined()) ? seed->data_ptr<int64_t>() : nullptr;
   const int64_t st[16] = {q.stride(0), q.stride(1), k.stride(0), k.stride(1), v.stride(0), v.stride(1), out.stride(0),
                           out.stride(1), go.stride(0), go.stride(1), dq.stride(0), dq.stride(1), dk.stride(0), dk.stride(1),
@@ -476,12 +478,7 @@ std::vector<at::Tensor> small_attention_backward(const at::Tensor& q, const at::
 // lse [B, H, Lq]}.
 static const uint8_t* dense_key_pad(const c10::optional<at::Tensor>& key_pad, at::Tensor& kpc, int64_t B, int64_t Lk,
                                     const at::Tensor& q) {
-  if (!key_pad.has_value() || !key_pad->defined()) return nullptr;
-  kpc = key_pad->contiguous();
-  TORCH_CHECK(kpc.device() == q.device() && kpc.dim() == 2 && kpc.size(0) == B && kpc.size(1) == Lk &&
-                  kpc.element_size() == 1,
-              "dense_attention: key_pad must be a bool [B, Lk] tensor on the device of q");
-  return static_cast<const uint8_t*>(kpc.data_ptr());
+  return checked_key_pad(key_pad, kpc, B, Lk, q, "dense_attention");
 }
 static void check_dense_shapes(const at::Tensor& q, const at::Tensor& k, const at::Tensor& v) {
   check_view(q, "q"); check_view(k, "k"); check_view(v, "v");

@@ -2,8 +2,10 @@
 
 Replaces the three-op forward / four-op backward chain the reference's transformer layers execute for every
 residual connection (src/trackformer/models/deformable_transformer.py:284-285, 291-292, 360-361, 370-371,
-377-378).  Same arithmetic (biased variance, eps inside the rsqrt, inverted dropout scaling 1/(1-p)); the
-dropout mask is drawn with torch's generator (graph-capture safe) and consumed by the kernel.
+377-378).  Same arithmetic (biased variance, eps inside the rsqrt, inverted dropout scaling 1/(1-p)).  In training
+the dropout mask is never stored: the kernels keep element ``row * C + c`` iff a hash of that index and a per-call
+int64 seed (``seeds.next_seed``, graph-capture safe) falls below ``keep * 2^32``, and the backward recomputes it from
+the same seed.  ``TFB200_LN_SEEDED=0`` switches to a bool mask drawn with torch's generator and read by the kernel.
 CUDA only -- on other devices / unsupported widths it defers to the stock PyTorch ops of the wrapped modules
 (that is the same arithmetic, not a different implementation of the MSDeformAttn core).
 """
