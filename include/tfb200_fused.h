@@ -173,6 +173,33 @@ int tfb200_set_loss_fwd_masked_f32(const float* logits, const float* boxes, cons
 int tfb200_set_loss_bwd_f32(const float* unit_logits, const float* unit_l1, const float* unit_giou, const float* g_ce,
                             const float* g_l1, const float* g_giou, const float* num_boxes, float* grad_logits,
                             float* grad_boxes, int K, int B, int Q, int C, void* stream);
+/* The same with the softmax classifier (focal_loss: false; models/matcher.py:77, models/detr.py:172-211).  Logits have
+ * C = classes + 1 columns, the last one "no object" (C >= 2).
+ *   match_cost_softmax / match_cost_track_softmax: class cost -softmax(logit_r)[label_t] (one log-sum-exp per row);
+ *                      otherwise as match_cost / match_cost_track.
+ *   set_loss_fwd_softmax: the weighted cross-entropy of loss_labels: target = matched label with weight 1, else no
+ *                      object with weight eos_coef (> 0); loss_ce[k] = sum_r w_r ce_r / sum_r w_r.  row_valid [B*Q]
+ *                      (optional) as in set_loss_fwd_masked.  row_pin [B*Q] (optional, see match_cost_track): when
+ *                      given, a valid unmatched row with pin -2 (false-positive track query) has its ce scaled by
+ *                      1 / eos_coef and counts 1 in the normaliser.  out6k[6][K] = out5k rows + the normaliser sum_r
+ *                      w_r; row_norm [R] is scratch.  Box terms, cardinality_error and class_error as set_loss_fwd.
+ *   set_loss_bwd_softmax: set_loss_bwd with the logit gradient scaled by g_ce[k] / ce_norm[k] (ce_norm = out6k + 5K). */
+int tfb200_match_cost_softmax_f32(const float* logits, const float* boxes, const int64_t* tgt_ids,
+                                  const float* tgt_boxes, float* cost, int64_t R, int C, int T, float w_class,
+                                  float w_bbox, float w_giou, void* stream);
+int tfb200_match_cost_track_softmax_f32(const float* logits, const float* boxes, const int64_t* tgt_ids,
+                                        const float* tgt_boxes, const int* row_pin, float* cost, int K, int B, int Q,
+                                        int C, int T, float w_class, float w_bbox, float w_giou, void* stream);
+int tfb200_set_loss_fwd_softmax_f32(const float* logits, const float* boxes, const int64_t* src, const int64_t* tgt,
+                                    const int64_t* tgt_ids, const float* tgt_boxes, const int* offsets,
+                                    const float* n_gt, const float* num_boxes, const uint8_t* row_valid,
+                                    const int* row_pin, float* unit_logits, float* unit_l1, float* unit_giou,
+                                    float* row_loss, float* row_norm, int* row_flags, float* pair_l1, float* pair_giou,
+                                    float* out6k, int K, int B, int Q, int C, int T, float eos_coef, void* stream);
+int tfb200_set_loss_bwd_softmax_f32(const float* unit_logits, const float* unit_l1, const float* unit_giou,
+                                    const float* g_ce, const float* g_l1, const float* g_giou, const float* num_boxes,
+                                    const float* ce_norm, float* grad_logits, float* grad_boxes, int K, int B, int Q,
+                                    int C, void* stream);
 
 /* Stem of the ResNet trunk in one pass (csrc/frozen_bn_act.cu): y = maxpool 3x3 / stride 2 / pad 1 of
  * relu(x * scale[c] + shift[c]); x [N][H][W][C] channels-last, y [N][(H+1)/2][(W+1)/2][C]; forward only (frozen stem). */

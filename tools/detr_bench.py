@@ -18,6 +18,12 @@ tracking latency.  Prints one JSON line with the card name and power limit (and 
                 graphed TrainStep (forward / backward CUDA graphs, loss in between, no optimizer) with the
                 dense-attention kernels on (TFB200_DENSE_ATTN=1) and off (the stock nn.MultiheadAttention), alternated
                 window by window in one process.  The eager arms are host-bound; the graphed one measures the GPU work.
+                Then, dense attention on, where the softmax SetCriterion runs, alternated window by window:
+                  one_graph   TrainStep(..., example_targets=...): forward, matching cost, device Hungarian matching,
+                              fused loss and backward replayed from ONE graph
+                  two_graph   forward / backward graphs with the device matching and the fused loss between them
+                  host_match  the same two graphs with scipy on the host (criterion.device_matcher = False): one
+                              device -> host copy of the cost per step
 --parts mots    Per-frame latency of DETRSegmTracking (20-class head, masks) at 1080x1920 through GraphedDetector +
                 DeviceTracker (host frame in, results out, device synchronised), --frames frames after --warmup.
 """
@@ -190,6 +196,22 @@ def bench_model(args, dev, result):
         dense_attention._ENABLED = True
         row[name + "_ms_dense_attn_on"] = statistics.median(times[True])
         row[name + "_ms_dense_attn_off"] = statistics.median(times[False])
+
+    dense_attention._ENABLED = True
+    host_criterion = copy.deepcopy(criterion)
+    host_criterion.device_matcher = False
+    arms = {"one_graph": TrainStep(copy.deepcopy(model).train(), criterion, None, use_graphs=True, example_frames=frame,
+                                   example_targets=targets),
+            "two_graph": graphed[True],
+            "host_match": TrainStep(copy.deepcopy(model).train(), host_criterion, None, use_graphs=True,
+                                    example_frames=frame)}
+    assert arms["one_graph"].g_full is not None, "the detection step was not captured into one graph"
+    times = {a: [] for a in arms}
+    for rep in range(args.repeats):
+        for a, st in arms.items():
+            times[a].append(time_ms(lambda st=st: st(frame, targets), args.iters, 1))
+    for a, v in times.items():
+        row[f"train_step_{a}_ms"] = statistics.median(v)
     result["model"] = row
     print("model", json.dumps(row), flush=True)
 

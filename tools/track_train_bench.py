@@ -4,7 +4,9 @@
 Workload: the tracking model (deformable DETR R50, 20-class head, random-init weights) trained on two-frame samples of
 `--height` x `--width` (default 800x1333, the geometry of BASELINE.json configs[2]) with 300 object queries, or with
 `--multi-frame` the documented training model (default_args(tracking=True, multi_frame=True): 500 queries, hidden 288,
-multi-frame attention, 8 levels).  Synthetic previous / current targets carry `--boxes` boxes per frame with shared
+multi-frame attention, 8 levels), or with `--vanilla` the vanilla-DETR tracking model (vanilla_args(tracking=True):
+cfgs/train.yaml + train_tracking.yaml, 100 object queries, dense attention, a 21-class softmax head, whose
+SetCriterion is the weighted cross-entropy one).  Synthetic previous / current targets carry `--boxes` boxes per frame with shared
 identities, so the previous frame's matching keeps enough identities for about `--tracks` track queries; the CPU
 generator is re-seeded before every step with a seed whose first two bookkeeping draws (detr_tracking.py: how many
 matches survive, how many false positives) give that count, so every timed step has the same K.
@@ -95,23 +97,36 @@ def main():
     ap.add_argument("--height", type=int, default=800)
     ap.add_argument("--width", type=int, default=1333)
     ap.add_argument("--batch", type=int, default=1)
-    ap.add_argument("--boxes", type=int, default=120)
-    ap.add_argument("--tracks", type=int, default=100)
+    ap.add_argument("--boxes", type=int, default=None, help="boxes per frame (default 120; 60 with --vanilla)")
+    ap.add_argument("--tracks", type=int, default=None, help="track queries (default 100; 50 with --vanilla)")
     ap.add_argument("--bucket", type=int, default=32)
     ap.add_argument("--multi-frame", action="store_true")
+    ap.add_argument("--vanilla", action="store_true", help="vanilla-DETR tracking model (softmax classifier)")
     ap.add_argument("--no-tf32", action="store_true")
     ap.add_argument("--check", action="store_true", help="dropout 0; compare both arms on the same seeded step")
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "track_train_bench needs a CUDA device"
+    if args.vanilla and args.multi_frame:
+        ap.error("--vanilla and --multi-frame are different models")
+    if args.boxes is None:
+        args.boxes = 60 if args.vanilla else 120
+    if args.tracks is None:
+        args.tracks = 50 if args.vanilla else 100
     from trackformer_b200.flat_adamw import reference_param_groups
-    from trackformer_b200.model_factory import build_model, default_args
+    from trackformer_b200.model_factory import build_model, default_args, vanilla_args
     from trackformer_b200.train_step import TrainStep
 
+    overrides = {"dropout": 0.0} if args.check else {}
+    model_args = vanilla_args(tracking=True, dataset="mot", device="cuda:0", **overrides) if args.vanilla \
+        else default_args(True, args.multi_frame, device="cuda:0", **overrides)
+    if args.boxes > model_args.num_queries:
+        ap.error(f"--boxes {args.boxes} exceeds the model's {model_args.num_queries} object queries")
+    if not torch.cuda.is_available():
+        sys.exit(f"track_train_bench needs a CUDA device (workload: {args.batch} x {args.height}x{args.width}, "
+                 f"{model_args.num_queries} queries, {args.boxes} boxes, ~{args.tracks} track queries)")
     dev = torch.device("cuda:0")
     torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = not args.no_tf32
-    overrides = {"dropout": 0.0} if args.check else {}
     torch.manual_seed(0)
-    model_a, criterion, _ = build_model(default_args(True, args.multi_frame, device="cuda:0", **overrides))
+    model_a, criterion, _ = build_model(model_args)
     model_a.to(dev).train()
     criterion.to(dev).train()
     prepare = getattr(model_a.backbone[0], "prepare", None)
@@ -142,8 +157,10 @@ def main():
     step = TrainStep(model_b, criterion, None, max_norm=0.1, use_graphs=True, example_frames=frames,
                      flat_adamw={"groups": reference_param_groups(model_b)}, track_bucket=args.bucket)
 
-    result = {"workload": "tracking train step, " + ("multi-frame model (500 queries, hidden 288, 8 levels)"
-                                                     if args.multi_frame else "300 object queries, 4 levels"),
+    workload = ("vanilla DETR (100 object queries, softmax classifier, 21 classes)" if args.vanilla else
+                "multi-frame model (500 queries, hidden 288, 8 levels)" if args.multi_frame else
+                "300 object queries, 4 levels")
+    result = {"workload": "tracking train step, " + workload,
               "frame": [args.height, args.width], "batch": args.batch, "boxes": args.boxes, "track_bucket": args.bucket,
               "tf32": not args.no_tf32, "dropout": 0.0 if args.check else 0.1}
 
@@ -171,7 +188,11 @@ def main():
         cos = float((ga * gb).sum() / (ga.norm() * gb.norm()).clamp_min(1e-30))
         loss_rel = abs(float(la) - float(lb)) / max(abs(float(la)), 1e-12)
         ok = same_idx and loss_rel < 1e-3 and rel < 2e-2 and cos > 0.999
+        differing = {k: int((x[k].long() != y[k].long()).sum()) if x[k].shape == y[k].shape else "shape"
+                     for x, y in zip(ta, tb)
+                     for k in ("track_query_match_ids", "track_queries_mask", "track_queries_fal_pos_mask")}
         result["check"] = {"ok": ok, "track_queries": len(ta[0]["track_query_boxes"]), "indices_equal": same_idx,
+                           "differing_entries": differing,
                            "loss_eager": float(la), "loss_graphed": float(lb), "loss_rel_diff": loss_rel,
                            "grad_sample_rel_l2": rel, "grad_sample_cosine": cos}
         if not ok:

@@ -102,6 +102,31 @@ class _SetLoss(torch.autograd.Function):
                                               num_boxes)
         return gl, gb, None, None, None, None, None, None, None, None, None, None
 
+
+class _SetLossSoftmax(torch.autograd.Function):
+    """``_SetLoss`` with the weighted cross-entropy of the softmax classifier: loss_ce[k] is normalised by the layer's
+    own weight sum (returned by the forward kernel, read by the backward one); ``row_pin`` (optional) marks the
+    false-positive track queries that keep their full weight."""
+    @staticmethod
+    def forward(ctx, logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets, n_gt, num_boxes, eos_coef, row_valid, row_pin):
+        from . import ext
+        out, ul, u1, ug = ext.load().set_loss_forward_softmax(logits, boxes, src, tgt, tgt_ids, tgt_boxes, offsets, n_gt,
+                                                              num_boxes, row_valid, row_pin, eos_coef)
+        ctx.save_for_backward(ul, u1, ug, num_boxes, out[5])
+        ce, l1, giou, card, cerr = out[:5].unbind(0)
+        ctx.mark_non_differentiable(card, cerr)
+        return ce, l1, giou, card, cerr
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_ce, g_l1, g_giou, _g_card, _g_err):
+        from . import ext
+        ul, u1, ug, num_boxes, ce_norm = ctx.saved_tensors
+        gl, gb = ext.load().set_loss_backward_softmax(ul, u1, ug, g_ce.contiguous(), g_l1.contiguous(),
+                                                      g_giou.contiguous(), num_boxes, ce_norm)
+        return gl, gb, None, None, None, None, None, None, None, None, None, None
+
+
 class LossDict(dict):
     """The loss dictionary of ``SetCriterion.forward_stacked`` (reference keys, detr.py:404-424) that also carries the
     per-layer loss VECTORS ``stacked = (loss_ce [K], loss_bbox [K], loss_giou [K])`` its entries are views of: a
@@ -260,7 +285,15 @@ class SetCriterion(nn.Module):
             return out
         return t
 
-    def _fused_losses(self, logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes, row_valid=None):
+    def _false_positive_pins(self, targets, nq, device):
+        """``row_pin`` of the matcher when false-positive track queries keep their full class weight (detr.py:190-197:
+        ``tracking`` and ``track_query_false_positive_eos_weight``), else None.  A valid row with pin -2 is one."""
+        if not (self.tracking and self.track_query_false_positive_eos_weight):
+            return None
+        return self.matcher.row_pin(targets, nq, device)
+
+    def _fused_losses(self, logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes, row_valid=None,
+                      row_pin=None):
         """The loss values of ``forward_stacked`` and their gradients from three launches (csrc/set_loss.cu)."""
         k = logits.shape[0]
         dev = logits.device
@@ -275,9 +308,14 @@ class SetCriterion(nn.Module):
             num_boxes = torch.tensor(float(num_boxes), dtype=torch.float32, device=dev)
         tgt_ids = torch.cat([t["labels"] for t in targets])
         tgt_boxes = torch.cat([t["boxes"] for t in targets]).float()
-        ce, l1, gi, card, cerr = _SetLoss.apply(logits, boxes, src2d, tgt2d, tgt_ids, tgt_boxes, off, n_gt,
-                                                num_boxes.reshape(1).float(), float(self.focal_alpha),
-                                                float(self.focal_gamma), row_valid)
+        if self.focal_loss:
+            ce, l1, gi, card, cerr = _SetLoss.apply(logits, boxes, src2d, tgt2d, tgt_ids, tgt_boxes, off, n_gt,
+                                                    num_boxes.reshape(1).float(), float(self.focal_alpha),
+                                                    float(self.focal_gamma), row_valid)
+        else:
+            ce, l1, gi, card, cerr = _SetLossSoftmax.apply(logits, boxes, src2d, tgt2d, tgt_ids, tgt_boxes, off, n_gt,
+                                                           num_boxes.reshape(1).float(), float(self.eos_coef),
+                                                           row_valid, row_pin)
         losses = LossDict({"loss_ce": ce[-1], "class_error": cerr[-1], "loss_bbox": l1[-1], "loss_giou": gi[-1],
                            "cardinality_error": card[-1]})
         for i in range(k - 1):
@@ -299,18 +337,22 @@ class SetCriterion(nn.Module):
         ``track_queries=True`` opts tracking targets (``track_query_match_ids`` ...) into this pass instead of the
         fallback: the track-query forcing of the matcher applies to every layer (on the device when it can, else on
         the host), and ``track_query_padding [Kb]`` (True = filler row, as fed to the decoder) marks rows that are
-        neither matched nor scored -- they add nothing to any loss and get no gradient, and the focal loss is
-        normalised as in the unpadded model."""
+        neither matched nor scored -- they add nothing to any loss and get no gradient, and the class loss is
+        normalised as in the unpadded model.
+
+        Both classifiers take this pass: the sigmoid focal loss (``focal_loss``) and the weighted cross-entropy of the
+        softmax classifier, whose false-positive track queries keep their full weight when ``tracking`` and
+        ``track_query_false_positive_eos_weight`` are set (detr.py:190-197)."""
         k, bs, nq, _ = logits.shape
         layers = [{"pred_logits": logits[i], "pred_boxes": boxes[i]} for i in range(k)]
         with_masks = "masks" in self.losses
-        special = (not self.focal_loss or set(self.losses) - {"masks"} != {"labels", "boxes", "cardinality"}
+        special = (set(self.losses) - {"masks"} != {"labels", "boxes", "cardinality"}
                    or not hasattr(self.matcher, "match_layers"))
         forced = track_queries and any("track_query_match_ids" in t or "track_query_padding" in t for t in targets)
         sizes = [len(t["labels"]) for t in targets]
         if forced and (special or with_masks or not hasattr(self.matcher, "match_layers_forced")):
             if any("track_query_padding" in t for t in targets):
-                raise NotImplementedError("filler track-query rows need the focal box-only criterion")
+                raise NotImplementedError("filler track-query rows need the box-only criterion")
             forced = False
         if not forced and (special or any("track_query_match_ids" in t for t in targets)
                            or min(sizes) == 0 or max(sizes) > nq):
@@ -366,30 +408,48 @@ class SetCriterion(nn.Module):
         if with_masks:
             last = slice((k - 1) * per_layer, None)
             masks = mask_losses(pred_masks, bat[last] * nq + src[last], tgt[last], targets, num_boxes)
+        row_pin = self._false_positive_pins(targets, nq, dev) if forced and not self.focal_loss else None
         if device_match is not None and _FUSED_LOSS and logits.dtype == torch.float32:
             losses = self._fused_losses(logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes,
-                                        None if row_valid is None else row_valid.reshape(-1).to(torch.uint8))
+                                        None if row_valid is None else row_valid.reshape(-1).to(torch.uint8), row_pin)
             if with_masks:
                 losses.update(masks)
             return losses
         gt_labels = torch.cat([t["labels"] for t in targets])[tgt]
         gt_boxes = torch.cat([t["boxes"] for t in targets])[tgt]
 
-        # labels: sigmoid focal loss against one-hot targets (no-object = all zeros)
         classes = torch.full((k, bs, nq), self.num_classes, dtype=torch.int64, device=dev)
         classes[lay, bat, src] = gt_labels
-        onehot = torch.zeros((k, bs, nq, logits.shape[-1] + 1), dtype=logits.dtype, device=dev)
-        onehot.scatter_(3, classes.unsqueeze(-1), 1)
-        onehot = onehot[..., :-1]
-        p = logits.sigmoid()
-        ce = F.binary_cross_entropy_with_logits(logits, onehot, reduction="none")
-        p_t = p * onehot + (1 - p) * (1 - onehot)
-        focal = ce * ((1 - p_t) ** self.focal_gamma)
-        if self.focal_alpha >= 0:
-            focal = (self.focal_alpha * onehot + (1 - self.focal_alpha) * (1 - onehot)) * focal
-        if row_valid is not None:
-            focal = focal * row_valid[None, :, :, None].to(focal.dtype)
-        loss_ce = focal.mean(2).sum((1, 2)) / num_boxes * nq                                   # [K]
+        if self.focal_loss:
+            # labels: sigmoid focal loss against one-hot targets (no-object = all zeros)
+            onehot = torch.zeros((k, bs, nq, logits.shape[-1] + 1), dtype=logits.dtype, device=dev)
+            onehot.scatter_(3, classes.unsqueeze(-1), 1)
+            onehot = onehot[..., :-1]
+            p = logits.sigmoid()
+            ce = F.binary_cross_entropy_with_logits(logits, onehot, reduction="none")
+            p_t = p * onehot + (1 - p) * (1 - onehot)
+            focal = ce * ((1 - p_t) ** self.focal_gamma)
+            if self.focal_alpha >= 0:
+                focal = (self.focal_alpha * onehot + (1 - self.focal_alpha) * (1 - onehot)) * focal
+            if row_valid is not None:
+                focal = focal * row_valid[None, :, :, None].to(focal.dtype)
+            loss_ce = focal.mean(2).sum((1, 2)) / num_boxes * nq                                   # [K]
+        else:
+            # labels: weighted cross-entropy (detr.py:185-204), each layer normalised by its own weight sum
+            weight = self.empty_weight.to(device=dev, dtype=logits.dtype)
+            ce = F.cross_entropy(logits.flatten(0, 2), classes.flatten(), weight=weight,
+                                 reduction="none").view(k, bs, nq)
+            w = weight[classes]
+            if row_pin is not None:                      # false-positive track queries: full weight, class-0 normaliser
+                fal_pos = row_pin.to(dev).view(bs, nq) == -2
+                if row_valid is not None:
+                    fal_pos = fal_pos & row_valid
+                ce = torch.where(fal_pos, ce * (1 / self.eos_coef), ce)
+                w = torch.where(fal_pos, weight[0], w)
+            if row_valid is not None:
+                ce = ce * row_valid.to(ce.dtype)
+                w = w * row_valid.to(w.dtype)
+            loss_ce = ce.sum((1, 2)) / w.sum((1, 2))                                                # [K]
 
         # boxes: L1 + GIoU over the matched pairs of every layer
         matched = boxes[lay, bat, src]

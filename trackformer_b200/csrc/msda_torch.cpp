@@ -742,6 +742,113 @@ std::vector<at::Tensor> set_loss_forward_masked(const at::Tensor& logits, const 
   return {out, ul, u1, ug};
 }
 
+// ---- the same with the softmax classifier (C = classes + 1, last column "no object") -------------------------------------
+// logits [..., C], boxes [..., 4] -> cost [R, T]
+at::Tensor match_cost_softmax(const at::Tensor& logits, const at::Tensor& boxes, const at::Tensor& tgt_ids,
+                              const at::Tensor& tgt_boxes, double w_class, double w_bbox, double w_giou) {
+  TORCH_CHECK(logits.is_cuda() && boxes.is_cuda() && tgt_ids.is_cuda() && tgt_boxes.is_cuda(),
+              "match_cost_softmax: CUDA tensors expected");
+  TORCH_CHECK(logits.scalar_type() == at::kFloat && boxes.scalar_type() == at::kFloat &&
+              tgt_ids.scalar_type() == at::kLong && tgt_boxes.scalar_type() == at::kFloat, "match_cost_softmax: dtypes");
+  const at::Tensor lg = logits.contiguous(), bx = boxes.contiguous(), ti = tgt_ids.contiguous(), tb = tgt_boxes.contiguous();
+  const int64_t C = lg.size(-1), R = lg.numel() / C, T = ti.numel();
+  TORCH_CHECK(bx.numel() == R * 4 && tb.numel() == T * 4 && T > 0 && C > 1, "match_cost_softmax: shapes");
+  const c10::cuda::CUDAGuard guard(logits.device());
+  at::Tensor cost = at::empty({R, T}, lg.options());
+  const int rc = tfb200_match_cost_softmax_f32(lg.data_ptr<float>(), bx.data_ptr<float>(), ti.data_ptr<int64_t>(),
+                                               tb.data_ptr<float>(), cost.data_ptr<float>(), R, int(C), int(T),
+                                               float(w_class), float(w_bbox), float(w_giou),
+                                               c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "match_cost_softmax failed (code ", rc, ")");
+  return cost;
+}
+
+// logits [K,B,Q,C], boxes [K,B,Q,4], row_pin int32 [B*Q] -> cost [K,B,Q,T] with the track-query forcing applied
+at::Tensor match_cost_track_softmax(const at::Tensor& logits, const at::Tensor& boxes, const at::Tensor& tgt_ids,
+                                    const at::Tensor& tgt_boxes, const at::Tensor& row_pin, double w_class, double w_bbox,
+                                    double w_giou) {
+  TORCH_CHECK(logits.is_cuda() && boxes.is_cuda() && tgt_ids.is_cuda() && tgt_boxes.is_cuda() && row_pin.is_cuda(),
+              "match_cost_track_softmax: CUDA tensors expected");
+  TORCH_CHECK(logits.scalar_type() == at::kFloat && boxes.scalar_type() == at::kFloat && tgt_ids.scalar_type() == at::kLong &&
+              tgt_boxes.scalar_type() == at::kFloat && row_pin.scalar_type() == at::kInt,
+              "match_cost_track_softmax: dtypes");
+  TORCH_CHECK(logits.dim() == 4 && boxes.dim() == 4, "match_cost_track_softmax: logits / boxes must be [K,B,Q,.]");
+  const at::Tensor lg = logits.contiguous(), bx = boxes.contiguous(), ti = tgt_ids.contiguous(), tb = tgt_boxes.contiguous();
+  const at::Tensor pin = row_pin.contiguous();
+  const int64_t K = lg.size(0), B = lg.size(1), Q = lg.size(2), C = lg.size(3), T = ti.numel();
+  TORCH_CHECK(bx.size(0) == K && bx.size(1) == B && bx.size(2) == Q && bx.size(3) == 4 && tb.numel() == T * 4 && T > 0 &&
+              pin.numel() == B * Q && C > 1, "match_cost_track_softmax: shapes");
+  const c10::cuda::CUDAGuard guard(logits.device());
+  at::Tensor cost = at::empty({K, B, Q, T}, lg.options());
+  const int rc = tfb200_match_cost_track_softmax_f32(lg.data_ptr<float>(), bx.data_ptr<float>(), ti.data_ptr<int64_t>(),
+                                                     tb.data_ptr<float>(), pin.data_ptr<int>(), cost.data_ptr<float>(),
+                                                     int(K), int(B), int(Q), int(C), int(T), float(w_class),
+                                                     float(w_bbox), float(w_giou),
+                                                     c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "match_cost_track_softmax failed (code ", rc, ")");
+  return cost;
+}
+
+// weighted cross-entropy + boxes; row_valid uint8 [B*Q] (filler rows = 0) and row_pin int32 [B*Q] (false-positive track
+// queries at full weight) are optional.  Returns {out6k [6][K], unit_logits, unit_l1, unit_giou}; out6k[5] is the
+// per-layer class-loss normaliser set_loss_backward_softmax takes.
+std::vector<at::Tensor> set_loss_forward_softmax(const at::Tensor& logits, const at::Tensor& boxes, const at::Tensor& src,
+                                                 const at::Tensor& tgt, const at::Tensor& tgt_ids, const at::Tensor& tgt_boxes,
+                                                 const at::Tensor& offsets, const at::Tensor& n_gt, const at::Tensor& num_boxes,
+                                                 const c10::optional<at::Tensor>& row_valid,
+                                                 const c10::optional<at::Tensor>& row_pin, double eos_coef) {
+  TORCH_CHECK(logits.is_cuda() && logits.dim() == 4 && boxes.dim() == 4 && logits.scalar_type() == at::kFloat &&
+              boxes.scalar_type() == at::kFloat && src.scalar_type() == at::kLong && tgt.scalar_type() == at::kLong &&
+              tgt_ids.scalar_type() == at::kLong && tgt_boxes.scalar_type() == at::kFloat &&
+              offsets.scalar_type() == at::kInt && n_gt.scalar_type() == at::kFloat && num_boxes.scalar_type() == at::kFloat &&
+              num_boxes.is_cuda() && n_gt.is_cuda() && offsets.is_cuda(), "set_loss_forward_softmax: dtypes / devices");
+  TORCH_CHECK(!row_valid.has_value() || (row_valid->scalar_type() == at::kByte && row_valid->is_cuda()),
+              "set_loss_forward_softmax: row_valid must be a CUDA uint8 tensor");
+  TORCH_CHECK(!row_pin.has_value() || (row_pin->scalar_type() == at::kInt && row_pin->is_cuda()),
+              "set_loss_forward_softmax: row_pin must be a CUDA int32 tensor");
+  const at::Tensor lg = logits.contiguous(), bx = boxes.contiguous(), s = src.contiguous(), t = tgt.contiguous();
+  const at::Tensor ti = tgt_ids.contiguous(), tb = tgt_boxes.contiguous();
+  const at::Tensor rv = row_valid.has_value() ? row_valid->contiguous() : at::Tensor();
+  const at::Tensor rp = row_pin.has_value() ? row_pin->contiguous() : at::Tensor();
+  const int64_t K = lg.size(0), B = lg.size(1), Q = lg.size(2), C = lg.size(3), T = s.size(-1);
+  TORCH_CHECK(s.numel() == K * T && t.numel() == K * T && ti.numel() == T && tb.numel() == 4 * T && offsets.numel() == B + 1 &&
+              n_gt.numel() == B && (!rv.defined() || rv.numel() == B * Q) && (!rp.defined() || rp.numel() == B * Q),
+              "set_loss_forward_softmax: shapes");
+  const c10::cuda::CUDAGuard guard(logits.device());
+  at::Tensor out = at::empty({6, K}, lg.options());
+  at::Tensor ul = at::empty_like(lg), u1 = at::empty_like(bx), ug = at::empty_like(bx);
+  at::Tensor row_loss = at::empty({2, K * B * Q}, lg.options()), row_flags = at::empty({K * B * Q}, lg.options().dtype(at::kInt));
+  at::Tensor pl = at::zeros({K, T}, lg.options()), pg = at::zeros({K, T}, lg.options());
+  const int rc = tfb200_set_loss_fwd_softmax_f32(
+      lg.data_ptr<float>(), bx.data_ptr<float>(), s.data_ptr<int64_t>(), t.data_ptr<int64_t>(), ti.data_ptr<int64_t>(),
+      tb.data_ptr<float>(), offsets.data_ptr<int>(), n_gt.data_ptr<float>(), num_boxes.data_ptr<float>(),
+      rv.defined() ? rv.data_ptr<uint8_t>() : nullptr, rp.defined() ? rp.data_ptr<int>() : nullptr, ul.data_ptr<float>(),
+      u1.data_ptr<float>(), ug.data_ptr<float>(), row_loss.data_ptr<float>(), row_loss.data_ptr<float>() + K * B * Q,
+      row_flags.data_ptr<int>(), pl.data_ptr<float>(), pg.data_ptr<float>(), out.data_ptr<float>(), int(K), int(B), int(Q),
+      int(C), int(T), float(eos_coef), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "set_loss_forward_softmax failed (code ", rc, ")");
+  return {out, ul, u1, ug};
+}
+
+std::vector<at::Tensor> set_loss_backward_softmax(const at::Tensor& unit_logits, const at::Tensor& unit_l1,
+                                                  const at::Tensor& unit_giou, const at::Tensor& g_ce, const at::Tensor& g_l1,
+                                                  const at::Tensor& g_giou, const at::Tensor& num_boxes,
+                                                  const at::Tensor& ce_norm) {
+  const int64_t K = unit_logits.size(0), B = unit_logits.size(1), Q = unit_logits.size(2), C = unit_logits.size(3);
+  const at::Tensor a = g_ce.contiguous(), b = g_l1.contiguous(), c = g_giou.contiguous(), n = ce_norm.contiguous();
+  TORCH_CHECK(a.numel() == K && b.numel() == K && c.numel() == K && n.numel() == K && a.scalar_type() == at::kFloat &&
+              n.scalar_type() == at::kFloat, "set_loss_backward_softmax: gradient / normaliser vectors [K]");
+  const c10::cuda::CUDAGuard guard(unit_logits.device());
+  at::Tensor gl = at::empty_like(unit_logits), gb = at::empty_like(unit_l1);
+  const int rc = tfb200_set_loss_bwd_softmax_f32(unit_logits.data_ptr<float>(), unit_l1.data_ptr<float>(),
+                                                 unit_giou.data_ptr<float>(), a.data_ptr<float>(), b.data_ptr<float>(),
+                                                 c.data_ptr<float>(), num_boxes.data_ptr<float>(), n.data_ptr<float>(),
+                                                 gl.data_ptr<float>(), gb.data_ptr<float>(), int(K), int(B), int(Q), int(C),
+                                                 c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "set_loss_backward_softmax failed (code ", rc, ")");
+  return {gl, gb};
+}
+
 std::vector<at::Tensor> set_loss_backward(const at::Tensor& unit_logits, const at::Tensor& unit_l1, const at::Tensor& unit_giou,
                                           const at::Tensor& g_ce, const at::Tensor& g_l1, const at::Tensor& g_giou,
                                           const at::Tensor& num_boxes) {
@@ -1158,6 +1265,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("set_loss_backward", &set_loss_backward);
   m.def("match_cost_track", &match_cost_track);
   m.def("set_loss_forward_masked", &set_loss_forward_masked);
+  m.def("match_cost_softmax", &match_cost_softmax);
+  m.def("match_cost_track_softmax", &match_cost_track_softmax);
+  m.def("set_loss_forward_softmax", &set_loss_forward_softmax);
+  m.def("set_loss_backward_softmax", &set_loss_backward_softmax);
   m.def("sampling_prep_forward", &sampling_prep_forward);
   m.def("sampling_prep_backward", &sampling_prep_backward);
   m.def("small_attention_forward", &small_attention_forward);

@@ -153,19 +153,23 @@ class HungarianMatcher(nn.Module):
             return None
         tgt_ids = torch.cat([t["labels"] for t in targets])
         tgt_boxes = torch.cat([t["boxes"] for t in targets])
-        fused = _FUSED_LOSS and self.focal_loss and logits.dtype == torch.float32
+        fused = _FUSED_LOSS and logits.dtype == torch.float32
+        # focal: (alpha, gamma) after the weights; softmax: the weights alone
+        cls_args = (self.focal_alpha, self.focal_gamma) if self.focal_loss else ()
         if forced:
             pin = self.row_pin(targets, nq, logits.device)
             if fused:
-                cost = ext.load().match_cost_track(logits, boxes, tgt_ids, tgt_boxes.float(), pin, self.cost_class,
-                                                   self.cost_bbox, self.cost_giou, self.focal_alpha, self.focal_gamma)
+                fn = ext.load().match_cost_track if self.focal_loss else ext.load().match_cost_track_softmax
+                cost = fn(logits, boxes, tgt_ids, tgt_boxes.float(), pin, self.cost_class, self.cost_bbox,
+                          self.cost_giou, *cls_args)
             else:
                 cost = self._cost(logits.flatten(0, 2), boxes.flatten(0, 2), tgt_ids, tgt_boxes).view(k, bs, nq, -1)
                 cost = self.force_cost(cost, pin)
         elif fused:
             # the whole cost matrix in one launch (csrc/set_loss.cu) instead of ~25 elementwise kernels
-            cost = ext.load().match_cost(logits, boxes, tgt_ids, tgt_boxes.float(), self.cost_class, self.cost_bbox,
-                                         self.cost_giou, self.focal_alpha, self.focal_gamma).view(k, bs, nq, -1)
+            fn = ext.load().match_cost if self.focal_loss else ext.load().match_cost_softmax
+            cost = fn(logits, boxes, tgt_ids, tgt_boxes.float(), self.cost_class, self.cost_bbox, self.cost_giou,
+                      *cls_args).view(k, bs, nq, -1)
         else:
             cost = self._cost(logits.flatten(0, 2), boxes.flatten(0, 2), tgt_ids, tgt_boxes).view(k, bs, nq, -1)
         key = (tuple(sizes), logits.device)

@@ -395,14 +395,14 @@ class TrainStep:
         ``"eager"``   the reference composition -- model(frames, targets) + ``criterion.forward`` + backward into the flat
                       gradient -- for what the decomposed step does not cover: a previous-previous frame
                       (``prev_prev_image``), backpropagation through the previous frame, and criteria other than the
-                      focal box-only one;
+                      box-only ones (``labels`` / ``boxes`` / ``cardinality``, either classifier);
         ``"track"``   everything else: the decomposed step of ``_track_step``."""
         from .detr_tracking import DETRTrackingBase
         model, crit = self.model, self.criterion
         if (not isinstance(model, DETRTrackingBase) or not model.training or model._tracking or not targets
                 or "prev_image" not in targets[0]):
             return "detect"
-        if ("prev_prev_image" in targets[0] or model._backprop_prev_frame or not crit.focal_loss
+        if ("prev_prev_image" in targets[0] or model._backprop_prev_frame
                 or set(crit.losses) != {"labels", "boxes", "cardinality"}
                 or not hasattr(crit.matcher, "match_layers_forced")):
             return "eager"
