@@ -317,6 +317,31 @@ int tfb200_upsample_add_fwd_f32(const float* x, const float* a, float* out, int 
                                 int Ho, int Wo, int C, void* stream);
 int tfb200_upsample_add_bwd_f32(const float* dout, float* dx, float* da, int N, int per_image, int Hi, int Wi, int Ho,
                                 int Wo, int C, void* stream);
+/* Ragged variants of the three (the matched query rows of a training step): P rows over B images, image b owning
+ * rows row_offsets[b] .. row_offsets[b + 1] (int32 [B + 1] on the device: row_offsets[0] = 0, non-decreasing,
+ * row_offsets[B] = P -- not checked on the host, which never reads it).  An image may own no rows: its attention-key
+ * gradient and its per-image operand gradients are then zero.  Same kernels, arithmetic and summation order as the
+ * per_image entry points, which equal these with row_offsets[b] = b * per_image.  mask_attn: q [P][heads*32],
+ * w / ds_ws [P][heads][HW], k / dk [B][HW][heads*32].  group_norm_relu: addend [B][HW][C] is required, mean / rstd
+ * [P][groups], partial_ws [P][2][C].  upsample_add: x [P][Hi][Wi][C], a / da [B][Ho][Wo][C].  P = 0 is legal
+ * (forwards: no-ops; backwards: zero per-image gradients); B = 0 requires P = 0.                                    */
+int tfb200_mask_attn_rows_fwd_f32(const float* q, const float* k, const uint8_t* pad, const int32_t* row_offsets,
+                                  float* w, int B, int P, int HW, int heads, float scale, void* stream);
+int tfb200_mask_attn_rows_bwd_f32(const float* q, const float* k, const int32_t* row_offsets, const float* w,
+                                  const float* dw, float* ds_ws, float* dq, float* dk, int B, int P, int HW, int heads,
+                                  float scale, void* stream);
+int tfb200_group_norm_relu_rows_fwd_f32(const float* x, const float* addend, const int32_t* row_offsets,
+                                        const float* gamma, const float* beta, float* y, float* mean, float* rstd,
+                                        int B, int P, int64_t HW, int C, int groups, float eps, void* stream);
+int tfb200_group_norm_relu_rows_bwd_f32(const float* dy, const float* x, const float* addend,
+                                        const int32_t* row_offsets, const float* y, const float* gamma,
+                                        const float* mean, const float* rstd, float* dx, float* daddend,
+                                        float* daffine, float* partial_ws, int B, int P, int64_t HW, int C, int groups,
+                                        void* stream);
+int tfb200_upsample_add_rows_fwd_f32(const float* x, const float* a, const int32_t* row_offsets, float* out, int B,
+                                     int P, int Hi, int Wi, int Ho, int Wo, int C, void* stream);
+int tfb200_upsample_add_rows_bwd_f32(const float* dout, const int32_t* row_offsets, float* dx, float* da, int B, int P,
+                                     int Hi, int Wi, int Ho, int Wo, int C, void* stream);
 /* mask_loss: M matched pairs (logits row src[m] of [R][h][w], target mask tgt[m] of [T][Ht][Wt] bool).  The logits
  * are sampled bilinearly (align_corners=False) at every target pixel on the fly; out2 = {sigmoid focal loss (mean
  * over pixels), dice} summed over pairs and divided by the device scalar *num_boxes.  M == 0 gives zeros.

@@ -17,6 +17,11 @@ Arms, alternated in the same run, each timed as ms/step with a device synchronis
           bookkeeping, padded current frame from forward / backward graphs, forced device matching + fused loss,
           one-pass clip + AdamW
 
+`--masks` trains the segmentation variant of the chosen model (DeformableDETRSegmTracking, or DETRSegmTracking with
+`--vanilla`): the targets carry one mask per box, the eager arm runs the reference's all-row mask head, the graphed arm
+is TrainStep(masks=True), whose mask head runs on the matched rows only.  Every arm also reports its peak allocated
+memory over its timed windows (torch.cuda.max_memory_allocated, both models' weights and optimiser state included).
+
 `--check` (dropout 0): before timing, both arms take the same seeded step from the same weights; their track-query
 indices must be equal and their loss and a seeded gradient sample close.
 
@@ -47,8 +52,9 @@ def card():
         return torch.cuda.get_device_name(0), "unknown"
 
 
-def make_sample(g, dev, size, n_boxes, batch):
-    """current frame + targets with prev_image / prev_target; the previous frame drops 5 identities and has 5 new ones"""
+def make_sample(g, dev, size, n_boxes, batch, masks=False):
+    """current frame + targets with prev_image / prev_target; the previous frame drops 5 identities and has 5 new ones;
+    with ``masks`` every box of the current frame gets a mask (its interior, ragged)"""
     h, w = size
     frames = torch.randn(batch, 3, h, w, generator=g).to(dev)
     targets = []
@@ -63,6 +69,12 @@ def make_sample(g, dev, size, n_boxes, batch):
              "image_id": torch.tensor([0])}
         pt = {"boxes": prev_boxes, "labels": torch.zeros(n_boxes, dtype=torch.int64), "track_ids": prev_ids,
               "image_id": torch.tensor([0])}
+        if masks:
+            ys = torch.arange(h, dtype=torch.float32)[:, None] / h
+            xs = torch.arange(w, dtype=torch.float32)[None, :] / w
+            t["masks"] = torch.stack([((xs - cx).abs() <= bw / 2) & ((ys - cy).abs() <= bh / 2)
+                                      & (torch.rand(h, w, generator=g) > 0.1)
+                                      for cx, cy, bw, bh in boxes.tolist()])
         t = {k: v.to(dev) for k, v in t.items()}
         t["prev_target"] = {k: v.to(dev) for k, v in pt.items()}
         t["prev_image"] = torch.randn(3, h, w, generator=g).to(dev)
@@ -102,6 +114,7 @@ def main():
     ap.add_argument("--bucket", type=int, default=32)
     ap.add_argument("--multi-frame", action="store_true")
     ap.add_argument("--vanilla", action="store_true", help="vanilla-DETR tracking model (softmax classifier)")
+    ap.add_argument("--masks", action="store_true", help="the segmentation model (TrainStep(masks=True))")
     ap.add_argument("--no-tf32", action="store_true")
     ap.add_argument("--check", action="store_true", help="dropout 0; compare both arms on the same seeded step")
     args = ap.parse_args()
@@ -116,6 +129,8 @@ def main():
     from trackformer_b200.train_step import TrainStep
 
     overrides = {"dropout": 0.0} if args.check else {}
+    if args.masks:
+        overrides["masks"] = True
     model_args = vanilla_args(tracking=True, dataset="mot", device="cuda:0", **overrides) if args.vanilla \
         else default_args(True, args.multi_frame, device="cuda:0", **overrides)
     if args.boxes > model_args.num_queries:
@@ -134,7 +149,7 @@ def main():
         prepare()                                       # the memory formats TrainStep gives the other arm's copy
     model_b = copy.deepcopy(model_a)
     g = torch.Generator().manual_seed(1)
-    frames, targets = make_sample(g, dev, (args.height, args.width), args.boxes, args.batch)
+    frames, targets = make_sample(g, dev, (args.height, args.width), args.boxes, args.batch, args.masks)
     seed = seed_for(args.tracks, args.boxes, model_a._track_query_false_positive_prob)
 
     # eager reference composition
@@ -155,11 +170,14 @@ def main():
         return loss.detach()
 
     step = TrainStep(model_b, criterion, None, max_norm=0.1, use_graphs=True, example_frames=frames,
-                     flat_adamw={"groups": reference_param_groups(model_b)}, track_bucket=args.bucket)
+                     flat_adamw={"groups": reference_param_groups(model_b)}, track_bucket=args.bucket,
+                     masks=args.masks)
 
     workload = ("vanilla DETR (100 object queries, softmax classifier, 21 classes)" if args.vanilla else
                 "multi-frame model (500 queries, hidden 288, 8 levels)" if args.multi_frame else
                 "300 object queries, 4 levels")
+    if args.masks:
+        workload += ", with the mask head"
     result = {"workload": "tracking train step, " + workload,
               "frame": [args.height, args.width], "batch": args.batch, "boxes": args.boxes, "track_bucket": args.bucket,
               "tf32": not args.no_tf32, "dropout": 0.0 if args.check else 0.1}
@@ -215,15 +233,20 @@ def main():
     window("eager", args.warmup)
     window("graphed", args.warmup)
     times = {"eager": [], "graphed": []}
+    peak = {"eager": 0, "graphed": 0}
     for _ in range(args.rounds):
         for arm in ("eager", "graphed"):
+            torch.cuda.reset_peak_memory_stats(dev)
             ms, k = window(arm, args.steps)
             times[arm].append(ms)
+            peak[arm] = max(peak[arm], torch.cuda.max_memory_allocated(dev))
     med = {a: sorted(v)[len(v) // 2] for a, v in times.items()}
     name, limit = card()
     result.update({"track_queries": k, "ms_per_step_eager": med["eager"], "ms_per_step_graphed": med["graphed"],
                    "speedup": med["eager"] / med["graphed"], "windows_ms": times, "steps_per_window": args.steps,
-                   "graph_captures": step.track_captures, "gpu": name, "power_limit": limit})
+                   "graph_captures": step.track_captures, "gpu": name, "power_limit": limit,
+                   "peak_allocated_mib_eager": peak["eager"] / 2 ** 20,
+                   "peak_allocated_mib_graphed": peak["graphed"] / 2 ** 20})
     print(json.dumps(result))
 
 

@@ -131,8 +131,15 @@ class LossDict(dict):
     """The loss dictionary of ``SetCriterion.forward_stacked`` (reference keys, detr.py:404-424) that also carries the
     per-layer loss VECTORS ``stacked = (loss_ce [K], loss_bbox [K], loss_giou [K])`` its entries are views of: a
     training step can then form the weighted total with three launches instead of one multiply and one add per
-    (loss, layer) entry forward and again backward (~110 single-element launches per step at K = 6)."""
+    (loss, layer) entry forward and again backward (~110 single-element launches per step at K = 6).
+
+    ``matched = (bat, src, tgt)`` are the last layer's matched pairs as int64 device tensors, image after image: query
+    ``src[i]`` of image ``bat[i]`` against global target ``tgt[i]`` (boxes of all images concatenated);
+    ``matched_sizes`` are the host counts of pairs per image.  The mask loss reads only these pairs, so a training step
+    can run the mask head on those rows alone."""
     stacked = None
+    matched = None
+    matched_sizes = None
 
 
 class SetCriterion(nn.Module):
@@ -232,6 +239,10 @@ class SetCriterion(nn.Module):
         return table[loss](outputs, targets, indices, num_boxes, **kwargs)
 
     def forward(self, outputs, targets, num_boxes=None):
+        return self._forward(outputs, targets, num_boxes)[0]
+
+    def _forward(self, outputs, targets, num_boxes=None, masks=True):
+        """``forward`` -> (losses, the last layer's indices); ``masks=False`` leaves the mask losses out."""
         last = {k: v for k, v in outputs.items() if k != "aux_outputs"}
         aux_list = list(outputs.get("aux_outputs", ()))
         if hasattr(self.matcher, "match_layers"):
@@ -252,6 +263,8 @@ class SetCriterion(nn.Module):
 
         losses = {}
         for name in self.losses:
+            if name == "masks" and not masks:
+                continue
             losses.update(self.get_loss(name, outputs, targets, indices, num_boxes))
         for i, aux in enumerate(aux_list):
             for name in self.losses:
@@ -260,7 +273,20 @@ class SetCriterion(nn.Module):
                 kw = {"log": False} if name == "labels" else {}
                 part = self.get_loss(name, aux, targets, all_indices[i + 1], num_boxes, **kw)
                 losses.update({f"{k}_{i}": v for k, v in part.items()})
-        return losses
+        return losses, indices
+
+    @staticmethod
+    def _matched_of(indices, targets, device):
+        """``LossDict.matched`` / ``matched_sizes`` from per-image host indices [(src, tgt)]"""
+        sizes = [len(s) for s, _ in indices]
+        ofs, bat, tgt = 0, [], []
+        for b, ((_, j), t) in enumerate(zip(indices, targets)):
+            bat.append(torch.full((len(j),), b, dtype=torch.int64))
+            tgt.append(j.to(torch.int64) + ofs)
+            ofs += len(t["labels"])
+        src = torch.cat([s.to(torch.int64).cpu() for s, _ in indices])
+        idx = torch.stack([torch.cat(bat), src, torch.cat(tgt).cpu()]).to(device, non_blocking=True)
+        return (idx[0], idx[1], idx[2]), sizes
 
     # ------------------------------------------------------------------------------------------
     def _num_boxes(self, targets, device):
@@ -332,7 +358,8 @@ class SetCriterion(nn.Module):
         all layers instead of K passes (the reference loops, detr.py:404-424): one Hungarian transfer, one focal
         loss, one L1/GIoU evaluation.  Keys and values equal ``forward`` on the equivalent dict (up to fp32
         summation order); falls back to it for the cases that need per-layer bookkeeping.  With the ``masks`` loss,
-        ``pred_masks [B,Q,h,w]`` of the last layer is scored against the last layer's matching.
+        ``pred_masks [B,Q,h,w]`` of the last layer is scored against the last layer's matching; without
+        ``pred_masks`` the mask losses are left out, for a caller that scores the masks of ``LossDict.matched`` itself.
 
         ``track_queries=True`` opts tracking targets (``track_query_match_ids`` ...) into this pass instead of the
         fallback: the track-query forcing of the matcher applies to every layer (on the device when it can, else on
@@ -350,17 +377,22 @@ class SetCriterion(nn.Module):
                    or not hasattr(self.matcher, "match_layers"))
         forced = track_queries and any("track_query_match_ids" in t or "track_query_padding" in t for t in targets)
         sizes = [len(t["labels"]) for t in targets]
-        if forced and (special or with_masks or not hasattr(self.matcher, "match_layers_forced")):
+        if forced and (special or not hasattr(self.matcher, "match_layers_forced")):
             if any("track_query_padding" in t for t in targets):
                 raise NotImplementedError("filler track-query rows need the box-only criterion")
             forced = False
         if not forced and (special or any("track_query_match_ids" in t for t in targets)
                            or min(sizes) == 0 or max(sizes) > nq):
             out = dict(layers[-1])
-            if with_masks:
+            if with_masks and pred_masks is not None:
                 out["pred_masks"] = pred_masks
             out["aux_outputs"] = layers[:-1]
-            return self.forward(out, targets, num_boxes)
+            if not with_masks:
+                return self.forward(out, targets, num_boxes)
+            found, indices = self._forward(out, targets, num_boxes, masks=pred_masks is not None)
+            losses = LossDict(found)
+            losses.matched, losses.matched_sizes = self._matched_of(indices, targets, logits.device)
+            return losses
 
         dev = logits.device
         per_layer = sum(sizes)
@@ -405,15 +437,17 @@ class SetCriterion(nn.Module):
             idx = torch.stack([lay, bat, src, tgt]).to(dev, non_blocking=True)
             lay, bat, src, tgt = idx[0], idx[1], idx[2], idx[3]
             n_gt = torch.as_tensor(sizes, device=dev, dtype=torch.float)
-        if with_masks:
-            last = slice((k - 1) * per_layer, None)
+        last = slice((k - 1) * per_layer, None)
+        last_pairs = (bat[last], src[last].long(), tgt[last])
+        masks = {}
+        if with_masks and pred_masks is not None:
             masks = mask_losses(pred_masks, bat[last] * nq + src[last], tgt[last], targets, num_boxes)
         row_pin = self._false_positive_pins(targets, nq, dev) if forced and not self.focal_loss else None
         if device_match is not None and _FUSED_LOSS and logits.dtype == torch.float32:
             losses = self._fused_losses(logits, boxes, src2d, tgt2d, targets, sizes, n_gt, num_boxes,
                                         None if row_valid is None else row_valid.reshape(-1).to(torch.uint8), row_pin)
-            if with_masks:
-                losses.update(masks)
+            losses.update(masks)
+            losses.matched, losses.matched_sizes = last_pairs, sizes
             return losses
         gt_labels = torch.cat([t["labels"] for t in targets])[tgt]
         gt_boxes = torch.cat([t["boxes"] for t in targets])[tgt]
@@ -474,6 +508,6 @@ class SetCriterion(nn.Module):
             losses[f"loss_giou_{i}"] = loss_giou[i]
             losses[f"cardinality_error_{i}"] = card[i]
         losses.stacked = (loss_ce, loss_bbox, loss_giou)
-        if with_masks:
-            losses.update(masks)
+        losses.update(masks)
+        losses.matched, losses.matched_sizes = last_pairs, sizes
         return losses

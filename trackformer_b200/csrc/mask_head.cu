@@ -60,18 +60,46 @@ __device__ float block_max(float v, float* red) {
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// Which image a query row belongs to.  Uniform: image b owns rows [b * per_image, (b + 1) * per_image).  Ragged
+// (the matched rows of a training step): image b owns rows [off[b], off[b + 1]), off [B + 1] int32 on the device,
+// off[0] = 0, non-decreasing; an image may own no rows.  Every kernel below is written once against this interface,
+// so the uniform and the ragged entry points run the same arithmetic in the same order.
+struct UniformRows {
+  int per_image;
+  __device__ __forceinline__ int image(int r) const { return r / per_image; }
+  __device__ __forceinline__ int begin(int b) const { return b * per_image; }
+  __device__ __forceinline__ int count(int) const { return per_image; }
+};
+
+struct RaggedRows {
+  const int* off;
+  int B;
+  __device__ __forceinline__ int image(int r) const {   // last b with off[b] <= r (skips images without rows)
+    int lo = 0, hi = B;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (__ldg(off + mid) <= r) lo = mid; else hi = mid;
+    }
+    return lo;
+  }
+  __device__ __forceinline__ int begin(int b) const { return __ldg(off + b); }
+  __device__ __forceinline__ int count(int b) const { return __ldg(off + b + 1) - __ldg(off + b); }
+};
+
+// ------------------------------------------------------------------------------------------------------------------
 // MHAttentionMap core: w[b][q] = softmax over (h, p) of scale * q[b][q][h] . k[b][p][h], -inf where pad[b][p].
 // One softmax over all heads and pixels together, as the reference's F.softmax(weights.flatten(2), dim=-1)
 // (detr_segmentation.py:214): the heads of a query share one partition sum.  One CTA per (b, q); its q row
 // (heads * 32 floats) is staged in dynamic shared memory.
 constexpr int kAttnFwdThreads = 512;
 
+template <class Rows>
 __global__ void __launch_bounds__(kAttnFwdThreads)
 mask_attn_fwd_kernel(const float* __restrict__ q, const float* __restrict__ k, const uint8_t* __restrict__ pad,
-                     float* __restrict__ w, int Q, int HW, int heads, float scale) {
+                     float* __restrict__ w, Rows rows, int HW, int heads, float scale) {
   extern __shared__ float4 qs[];                    // [heads][kHeadDim / 4]
   __shared__ float red[32];
-  const int bq = blockIdx.x, b = bq / Q;
+  const int bq = blockIdx.x, b = rows.image(bq);
   const int D = heads * kHeadDim;
   for (int i = threadIdx.x; i < D / 4; i += blockDim.x)
     qs[i] = reinterpret_cast<const float4*>(q + int64_t(bq) * D)[i];
@@ -110,13 +138,14 @@ mask_attn_fwd_kernel(const float* __restrict__ q, const float* __restrict__ k, c
 // ds = w * (dw - sum(dw * w)) (softmax backward; the sum runs over the whole (b, q) row, all heads and pixels, as the
 // forward's softmax does), dq = scale * ds . k.  One CTA per (b, q, h): each of a row's CTAs computes the row sum
 // itself, in the same order, so they all use the same value.
+template <class Rows>
 __global__ void __launch_bounds__(256)
 mask_attn_bwd_dq_kernel(const float* __restrict__ k, const float* __restrict__ w, const float* __restrict__ dw,
-                        float* __restrict__ ds, float* __restrict__ dq, int Q, int HW, int heads, float scale) {
+                        float* __restrict__ ds, float* __restrict__ dq, Rows rows, int HW, int heads, float scale) {
   __shared__ float red[32];
   __shared__ float part[8][kHeadDim];
   const int row = blockIdx.x;
-  const int h = row % heads, bq = row / heads, b = bq / Q;
+  const int h = row % heads, bq = row / heads, b = rows.image(bq);
   const int D = heads * kHeadDim;
   const int64_t n = int64_t(heads) * HW;
   const float* wq = w + int64_t(bq) * n;
@@ -158,13 +187,16 @@ mask_attn_bwd_dq_kernel(const float* __restrict__ k, const float* __restrict__ w
   }
 }
 
-// dk[b][p][h][:] = scale * sum_q ds[b][q][h][p] * q[b][q][h][:]; grid (ceil(HW / 128), heads, B), thread per p
+// dk[b][p][h][:] = scale * sum_q ds[b][q][h][p] * q[b][q][h][:] over the rows q of image b, in row order (zero for
+// an image without rows); grid (ceil(HW / 128), heads, B), thread per p
+template <class Rows>
 __global__ void __launch_bounds__(128)
-mask_attn_bwd_dk_kernel(const float* __restrict__ q, const float* __restrict__ ds, float* __restrict__ dk, int Q,
+mask_attn_bwd_dk_kernel(const float* __restrict__ q, const float* __restrict__ ds, float* __restrict__ dk, Rows rows,
                         int HW, int heads, float scale) {
   __shared__ float qt[32][kHeadDim];
   const int p = blockIdx.x * 128 + threadIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int D = heads * kHeadDim;
+  const int r0 = rows.begin(b), Q = rows.count(b);
   float acc[kHeadDim];
 #pragma unroll
   for (int c = 0; c < kHeadDim; ++c) acc[c] = 0.f;
@@ -172,11 +204,11 @@ mask_attn_bwd_dk_kernel(const float* __restrict__ q, const float* __restrict__ d
     const int nq = min(32, Q - q0);
     __syncthreads();
     for (int i = threadIdx.x; i < nq * kHeadDim; i += 128)
-      qt[i / kHeadDim][i % kHeadDim] = q[(int64_t(b) * Q + q0 + i / kHeadDim) * D + h * kHeadDim + i % kHeadDim];
+      qt[i / kHeadDim][i % kHeadDim] = q[(int64_t(r0) + q0 + i / kHeadDim) * D + h * kHeadDim + i % kHeadDim];
     __syncthreads();
     if (p < HW) {
       for (int j = 0; j < nq; ++j) {
-        const float g = ds[((int64_t(b) * Q + q0 + j) * heads + h) * HW + p];
+        const float g = ds[((int64_t(r0) + q0 + j) * heads + h) * HW + p];
 #pragma unroll
         for (int c = 0; c < kHeadDim; ++c) acc[c] = fmaf(g, qt[j][c], acc[c]);
       }
@@ -196,10 +228,11 @@ mask_attn_bwd_dk_kernel(const float* __restrict__ q, const float* __restrict__ d
 // (affine gradients) stay in registers until one ordered reduction at the end.
 __device__ __forceinline__ int gn_threads(int cpg) { return cpg * (256 / cpg); }
 
+template <class Rows>
 __global__ void __launch_bounds__(256)
 group_norm_relu_fwd_kernel(const float* __restrict__ x, const float* __restrict__ addend,
                            const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ y,
-                           float* __restrict__ mean_out, float* __restrict__ rstd_out, int per_image, int64_t HW, int C,
+                           float* __restrict__ mean_out, float* __restrict__ rstd_out, Rows rows, int64_t HW, int C,
                            int groups, float eps) {
   __shared__ float red[32];
   const int n = blockIdx.x / groups, g = blockIdx.x % groups, cpg = C / groups;
@@ -208,7 +241,7 @@ group_norm_relu_fwd_kernel(const float* __restrict__ x, const float* __restrict_
   const int ch = g * cpg + threadIdx.x % cpg;
   const int64_t p0 = threadIdx.x / cpg, step = nt / cpg;
   const float* xs = x + int64_t(n) * HW * C + ch;
-  const float* as = addend != nullptr ? addend + int64_t(n / per_image) * HW * C + ch : nullptr;
+  const float* as = addend != nullptr ? addend + int64_t(rows.image(n)) * HW * C + ch : nullptr;
   float s = 0.f;
   if (active)
     for (int64_t p = p0; p < HW; p += step) s += xs[p * C] + (as ? as[p * C] : 0.f);
@@ -234,11 +267,12 @@ group_norm_relu_fwd_kernel(const float* __restrict__ x, const float* __restrict_
 }
 
 // dx of GroupNorm + ReLU, and per-sample affine partials partial[n][0][c] (dgamma) / partial[n][1][c] (dbeta)
+template <class Rows>
 __global__ void __launch_bounds__(256)
 group_norm_relu_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ addend,
                            const float* __restrict__ y, const float* __restrict__ gamma,
                            const float* __restrict__ mean_in, const float* __restrict__ rstd_in, float* __restrict__ dx,
-                           float* __restrict__ partial, int per_image, int64_t HW, int C, int groups) {
+                           float* __restrict__ partial, Rows rows, int64_t HW, int C, int groups) {
   __shared__ float red[32];
   __shared__ float pg[256], pb[256];
   const int n = blockIdx.x / groups, g = blockIdx.x % groups, cpg = C / groups;
@@ -247,7 +281,7 @@ group_norm_relu_bwd_kernel(const float* __restrict__ dy, const float* __restrict
   const int ch = g * cpg + threadIdx.x % cpg;
   const int64_t p0 = threadIdx.x / cpg, step = nt / cpg;
   const int64_t base = int64_t(n) * HW * C + ch;
-  const float* as = addend != nullptr ? addend + int64_t(n / per_image) * HW * C + ch : nullptr;
+  const float* as = addend != nullptr ? addend + int64_t(rows.image(n)) * HW * C + ch : nullptr;
   const float mean = mean_in[blockIdx.x], rstd = rstd_in[blockIdx.x];
   const float ga = active ? gamma[ch] : 0.f;
   float sd = 0.f, sdx = 0.f, dg = 0.f, db = 0.f;
@@ -294,15 +328,17 @@ __global__ void sum_rows_kernel(const float* __restrict__ in, float* __restrict_
   out[e] = t;
 }
 
-// out[b][e] = sum_q in[b * per_image + q][e]: gradient of an operand broadcast over the queries of an image
-__global__ void sum_queries_kernel(const float* __restrict__ in, float* __restrict__ out, int per_image,
-                                   int64_t inner) {
+// out[b][e] = sum over the rows q of image b of in[q][e], in row order (zero for an image without rows): gradient of
+// an operand broadcast over the queries of an image
+template <class Rows>
+__global__ void sum_queries_kernel(const float* __restrict__ in, float* __restrict__ out, Rows rows, int64_t inner) {
   const int64_t e = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (e >= inner) return;
   const int b = blockIdx.y;
-  const float* src = in + int64_t(b) * per_image * inner + e;
+  const float* src = in + int64_t(rows.begin(b)) * inner + e;
+  const int n = rows.count(b);
   float t = 0.f;
-  for (int q = 0; q < per_image; ++q) t += src[int64_t(q) * inner];
+  for (int q = 0; q < n; ++q) t += src[int64_t(q) * inner];
   out[int64_t(b) * inner + e] = t;
 }
 
@@ -315,8 +351,9 @@ __device__ __forceinline__ int nearest_src(int o, int in, int out) {
   return min(int(floorf(float(o) * scale)), in - 1);
 }
 
+template <class Rows>
 __global__ void upsample_add_fwd_kernel(const float* __restrict__ x, const float* __restrict__ a,
-                                        float* __restrict__ out, int per_image, int Hi, int Wi, int Ho, int Wo, int C,
+                                        float* __restrict__ out, Rows rows, int Hi, int Wi, int Ho, int Wo, int C,
                                         int64_t total) {
   const int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -327,7 +364,7 @@ __global__ void upsample_add_fwd_kernel(const float* __restrict__ x, const float
   const int ho = int(r % Ho);
   const int n = int(r / Ho);
   const int hi = nearest_src(ho, Hi, Ho), wi = nearest_src(wo, Wi, Wo);
-  out[i] = a[((int64_t(n / per_image) * Ho + ho) * Wo + wo) * C + c] + x[((int64_t(n) * Hi + hi) * Wi + wi) * C + c];
+  out[i] = a[((int64_t(rows.image(n)) * Ho + ho) * Wo + wo) * C + c] + x[((int64_t(n) * Hi + hi) * Wi + wi) * C + c];
 }
 
 // dx[n][hi][wi][c] = sum of dout over the output pixels whose nearest source is (hi, wi)
@@ -508,19 +545,107 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 // the attention forward stages a query's q row in shared memory: heads * 32 floats, at most 32 KiB
 constexpr int kMaxAttnHeads = 256;
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Launchers shared by the uniform (per_image) and the ragged (row_offsets) entry points: P query rows over B images.
+
+template <class Rows>
+int launch_attn_fwd(const float* q, const float* k, const uint8_t* pad, float* w, Rows rows, int P, int HW, int heads,
+                    float scale, cudaStream_t s) {
+  if (P == 0) return 0;
+  mask_attn_fwd_kernel<<<unsigned(P), kAttnFwdThreads, sizeof(float) * heads * kHeadDim, s>>>(q, k, pad, w, rows, HW,
+                                                                                             heads, scale);
+  msda_b200_count_launches(1);
+  return int(cudaGetLastError());
+}
+
+template <class Rows>
+int launch_attn_bwd(const float* q, const float* k, const float* w, const float* dw, float* ds_ws, float* dq, float* dk,
+                    Rows rows, int B, int P, int HW, int heads, float scale, cudaStream_t s) {
+  if (B == 0) return 0;
+  if (P == 0) return int(cudaMemsetAsync(dk, 0, sizeof(float) * size_t(B) * HW * heads * kHeadDim, s));
+  mask_attn_bwd_dq_kernel<<<unsigned(P * heads), 256, 0, s>>>(k, w, dw, ds_ws, dq, rows, HW, heads, scale);
+  mask_attn_bwd_dk_kernel<<<dim3(blocks_for(HW, 128), heads, B), 128, 0, s>>>(q, ds_ws, dk, rows, HW, heads, scale);
+  msda_b200_count_launches(2);
+  return int(cudaGetLastError());
+}
+
+int gn_check(int N, int64_t HW, int C, int groups) {
+  if (N < 0 || HW <= 0 || C <= 0 || groups <= 0 || C % groups != 0 || C / groups > 256) return TFB200_E_SHAPE;
+  return 0;
+}
+
+template <class Rows>
+int launch_gn_fwd(const float* x, const float* addend, const float* gamma, const float* beta, float* y, float* mean,
+                  float* rstd, Rows rows, int N, int64_t HW, int C, int groups, float eps, cudaStream_t s) {
+  if (N == 0) return 0;
+  group_norm_relu_fwd_kernel<<<unsigned(N * groups), 256, 0, s>>>(x, addend, gamma, beta, y, mean, rstd, rows, HW, C,
+                                                                  groups, eps);
+  msda_b200_count_launches(1);
+  return int(cudaGetLastError());
+}
+
+template <class Rows>
+int launch_gn_bwd(const float* dy, const float* x, const float* addend, const float* y, const float* gamma,
+                  const float* mean, const float* rstd, float* dx, float* daddend, float* daffine, float* partial_ws,
+                  Rows rows, int B, int N, int64_t HW, int C, int groups, cudaStream_t s) {
+  if (N == 0) {
+    cudaError_t e = cudaMemsetAsync(daffine, 0, 2 * sizeof(float) * C, s);
+    if (e == cudaSuccess && addend != nullptr && B > 0) e = cudaMemsetAsync(daddend, 0, sizeof(float) * B * HW * C, s);
+    return int(e);
+  }
+  group_norm_relu_bwd_kernel<<<unsigned(N * groups), 256, 0, s>>>(dy, x, addend, y, gamma, mean, rstd, dx, partial_ws,
+                                                                   rows, HW, C, groups);
+  // partial_ws is [N][2][C]: daffine = {dgamma, dbeta} is its sum over the samples
+  sum_rows_kernel<<<blocks_for(2 * C, 256), 256, 0, s>>>(partial_ws, daffine, N, int64_t(2 * C));
+  int launches = 2;
+  if (addend != nullptr && B > 0) {
+    const int64_t inner = HW * C;
+    sum_queries_kernel<<<dim3(blocks_for(inner, 256), B), 256, 0, s>>>(dx, daddend, rows, inner);
+    ++launches;
+  }
+  msda_b200_count_launches(launches);
+  return int(cudaGetLastError());
+}
+
+bool up_shape_ok(int Hi, int Wi, int Ho, int Wo, int C) { return Hi > 0 && Wi > 0 && Ho > 0 && Wo > 0 && C > 0; }
+
+template <class Rows>
+int launch_up_fwd(const float* x, const float* a, float* out, Rows rows, int N, int Hi, int Wi, int Ho, int Wo, int C,
+                  cudaStream_t s) {
+  const int64_t total = int64_t(N) * Ho * Wo * C;
+  if (total == 0) return 0;
+  upsample_add_fwd_kernel<<<blocks_for(total, 256), 256, 0, s>>>(x, a, out, rows, Hi, Wi, Ho, Wo, C, total);
+  msda_b200_count_launches(1);
+  return int(cudaGetLastError());
+}
+
+template <class Rows>
+int launch_up_bwd(const float* dout, float* dx, float* da, Rows rows, int B, int N, int Hi, int Wi, int Ho, int Wo,
+                  int C, cudaStream_t s) {
+  if (B == 0) return 0;
+  const int64_t total = int64_t(N) * Hi * Wi * C, inner = int64_t(Ho) * Wo * C;
+  int launches = 1;
+  if (total > 0) {
+    upsample_add_bwd_dx_kernel<<<blocks_for(total, 256), 256, 0, s>>>(dout, dx, Hi, Wi, Ho, Wo, C, total);
+    ++launches;
+  }
+  sum_queries_kernel<<<dim3(blocks_for(inner, 256), B), 256, 0, s>>>(dout, da, rows, inner);
+  msda_b200_count_launches(launches);
+  return int(cudaGetLastError());
+}
+
+// the ragged entry points: B >= 0 images owning P >= 0 rows in all
+inline bool rows_ok(int B, int P) { return B >= 0 && P >= 0 && (B > 0 || P == 0); }
+
 }  // namespace
 
-// ---------------------------------------------------------------------------------------------------------------------
 extern "C" int tfb200_mask_attn_fwd_f32(const float* q, const float* k, const uint8_t* pad, float* w, int B, int Q,
                                         int HW, int heads, float scale, void* stream) {
   if (!q || !k || !w) return TFB200_E_NULLPTR;
   if (B < 0 || Q < 0 || HW <= 0 || heads <= 0 || heads > kMaxAttnHeads || !aligned16(q) || !aligned16(k))
     return TFB200_E_SHAPE;
   if (int64_t(B) * Q == 0) return 0;
-  mask_attn_fwd_kernel<<<unsigned(B * Q), kAttnFwdThreads, sizeof(float) * heads * kHeadDim, cudaStream_t(stream)>>>(
-      q, k, pad, w, Q, HW, heads, scale);
-  msda_b200_count_launches(1);
-  return int(cudaGetLastError());
+  return launch_attn_fwd(q, k, pad, w, UniformRows{Q}, B * Q, HW, heads, scale, cudaStream_t(stream));
 }
 
 extern "C" int tfb200_mask_attn_bwd_f32(const float* q, const float* k, const float* w, const float* dw, float* ds_ws,
@@ -528,32 +653,36 @@ extern "C" int tfb200_mask_attn_bwd_f32(const float* q, const float* k, const fl
                                         void* stream) {
   if (!q || !k || !w || !dw || !ds_ws || !dq || !dk) return TFB200_E_NULLPTR;
   if (B < 0 || Q < 0 || HW <= 0 || heads <= 0 || !aligned16(k) || !aligned16(dk)) return TFB200_E_SHAPE;
-  if (B == 0) return 0;
-  const cudaStream_t s = cudaStream_t(stream);
-  if (Q == 0) return int(cudaMemsetAsync(dk, 0, sizeof(float) * size_t(B) * HW * heads * kHeadDim, s));
-  mask_attn_bwd_dq_kernel<<<unsigned(B * Q * heads), 256, 0, s>>>(k, w, dw, ds_ws, dq, Q, HW, heads, scale);
-  mask_attn_bwd_dk_kernel<<<dim3(blocks_for(HW, 128), heads, B), 128, 0, s>>>(q, ds_ws, dk, Q, HW, heads, scale);
-  msda_b200_count_launches(2);
-  return int(cudaGetLastError());
+  return launch_attn_bwd(q, k, w, dw, ds_ws, dq, dk, UniformRows{Q > 0 ? Q : 1}, B, B * Q, HW, heads, scale,
+                         cudaStream_t(stream));
 }
 
-static int gn_check(int N, int per_image, int64_t HW, int C, int groups) {
-  if (N < 0 || per_image <= 0 || HW <= 0 || C <= 0 || groups <= 0 || C % groups != 0 || C / groups > 256 ||
-      N % per_image != 0)
+extern "C" int tfb200_mask_attn_rows_fwd_f32(const float* q, const float* k, const uint8_t* pad,
+                                             const int32_t* row_offsets, float* w, int B, int P, int HW, int heads,
+                                             float scale, void* stream) {
+  if (!row_offsets || (P > 0 && (!q || !w)) || (B > 0 && !k)) return TFB200_E_NULLPTR;
+  if (!rows_ok(B, P) || HW <= 0 || heads <= 0 || heads > kMaxAttnHeads || !aligned16(q) || !aligned16(k))
     return TFB200_E_SHAPE;
-  return 0;
+  return launch_attn_fwd(q, k, pad, w, RaggedRows{row_offsets, B}, P, HW, heads, scale, cudaStream_t(stream));
+}
+
+extern "C" int tfb200_mask_attn_rows_bwd_f32(const float* q, const float* k, const int32_t* row_offsets, const float* w,
+                                             const float* dw, float* ds_ws, float* dq, float* dk, int B, int P, int HW,
+                                             int heads, float scale, void* stream) {
+  if (!row_offsets || (P > 0 && (!q || !w || !dw || !ds_ws || !dq)) || (B > 0 && (!k || !dk))) return TFB200_E_NULLPTR;
+  if (!rows_ok(B, P) || HW <= 0 || heads <= 0 || !aligned16(k) || !aligned16(dk)) return TFB200_E_SHAPE;
+  return launch_attn_bwd(q, k, w, dw, ds_ws, dq, dk, RaggedRows{row_offsets, B}, B, P, HW, heads, scale,
+                         cudaStream_t(stream));
 }
 
 extern "C" int tfb200_group_norm_relu_fwd_f32(const float* x, const float* addend, const float* gamma,
                                               const float* beta, float* y, float* mean, float* rstd, int N,
                                               int per_image, int64_t HW, int C, int groups, float eps, void* stream) {
   if (!x || !gamma || !beta || !y || !mean || !rstd) return TFB200_E_NULLPTR;
-  if (const int rc = gn_check(N, per_image, HW, C, groups)) return rc;
-  if (N == 0) return 0;
-  group_norm_relu_fwd_kernel<<<unsigned(N * groups), 256, 0, cudaStream_t(stream)>>>(
-      x, addend, gamma, beta, y, mean, rstd, per_image, HW, C, groups, eps);
-  msda_b200_count_launches(1);
-  return int(cudaGetLastError());
+  if (per_image <= 0 || N % per_image != 0) return TFB200_E_SHAPE;
+  if (const int rc = gn_check(N, HW, C, groups)) return rc;
+  return launch_gn_fwd(x, addend, gamma, beta, y, mean, rstd, UniformRows{per_image}, N, HW, C, groups, eps,
+                       cudaStream_t(stream));
 }
 
 extern "C" int tfb200_group_norm_relu_bwd_f32(const float* dy, const float* x, const float* addend, const float* y,
@@ -562,48 +691,65 @@ extern "C" int tfb200_group_norm_relu_bwd_f32(const float* dy, const float* x, c
                                               int per_image, int64_t HW, int C, int groups, void* stream) {
   if (!dy || !x || !y || !gamma || !mean || !rstd || !dx || !daffine || !partial_ws) return TFB200_E_NULLPTR;
   if (addend != nullptr && daddend == nullptr) return TFB200_E_NULLPTR;
-  if (const int rc = gn_check(N, per_image, HW, C, groups)) return rc;
-  const cudaStream_t s = cudaStream_t(stream);
-  if (N == 0) return int(cudaMemsetAsync(daffine, 0, 2 * sizeof(float) * C, s));
-  group_norm_relu_bwd_kernel<<<unsigned(N * groups), 256, 0, s>>>(dy, x, addend, y, gamma, mean, rstd, dx, partial_ws,
-                                                                   per_image, HW, C, groups);
-  // partial_ws is [N][2][C]: daffine = {dgamma, dbeta} is its sum over the samples
-  sum_rows_kernel<<<blocks_for(2 * C, 256), 256, 0, s>>>(partial_ws, daffine, N, int64_t(2 * C));
-  int launches = 2;
-  if (addend != nullptr) {
-    const int64_t inner = HW * C;
-    sum_queries_kernel<<<dim3(blocks_for(inner, 256), N / per_image), 256, 0, s>>>(dx, daddend, per_image, inner);
-    ++launches;
-  }
-  msda_b200_count_launches(launches);
-  return int(cudaGetLastError());
+  if (per_image <= 0 || N % per_image != 0) return TFB200_E_SHAPE;
+  if (const int rc = gn_check(N, HW, C, groups)) return rc;
+  return launch_gn_bwd(dy, x, addend, y, gamma, mean, rstd, dx, daddend, daffine, partial_ws, UniformRows{per_image},
+                       N / per_image, N, HW, C, groups, cudaStream_t(stream));
+}
+
+extern "C" int tfb200_group_norm_relu_rows_fwd_f32(const float* x, const float* addend, const int32_t* row_offsets,
+                                                   const float* gamma, const float* beta, float* y, float* mean,
+                                                   float* rstd, int B, int P, int64_t HW, int C, int groups, float eps,
+                                                   void* stream) {
+  if (!row_offsets || !gamma || !beta || (P > 0 && (!x || !y || !mean || !rstd)) || (B > 0 && !addend))
+    return TFB200_E_NULLPTR;
+  if (!rows_ok(B, P)) return TFB200_E_SHAPE;
+  if (const int rc = gn_check(P, HW, C, groups)) return rc;
+  return launch_gn_fwd(x, addend, gamma, beta, y, mean, rstd, RaggedRows{row_offsets, B}, P, HW, C, groups, eps,
+                       cudaStream_t(stream));
+}
+
+extern "C" int tfb200_group_norm_relu_rows_bwd_f32(const float* dy, const float* x, const float* addend,
+                                                   const int32_t* row_offsets, const float* y, const float* gamma,
+                                                   const float* mean, const float* rstd, float* dx, float* daddend,
+                                                   float* daffine, float* partial_ws, int B, int P, int64_t HW, int C,
+                                                   int groups, void* stream) {
+  if (!row_offsets || !gamma || !daffine || (P > 0 && (!dy || !x || !y || !mean || !rstd || !dx || !partial_ws)) ||
+      (B > 0 && (!addend || !daddend)))
+    return TFB200_E_NULLPTR;
+  if (!rows_ok(B, P)) return TFB200_E_SHAPE;
+  if (const int rc = gn_check(P, HW, C, groups)) return rc;
+  return launch_gn_bwd(dy, x, addend, y, gamma, mean, rstd, dx, daddend, daffine, partial_ws,
+                       RaggedRows{row_offsets, B}, B, P, HW, C, groups, cudaStream_t(stream));
 }
 
 extern "C" int tfb200_upsample_add_fwd_f32(const float* x, const float* a, float* out, int N, int per_image, int Hi,
                                            int Wi, int Ho, int Wo, int C, void* stream) {
   if (!x || !a || !out) return TFB200_E_NULLPTR;
-  if (N < 0 || per_image <= 0 || N % per_image != 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || C <= 0)
-    return TFB200_E_SHAPE;
-  const int64_t total = int64_t(N) * Ho * Wo * C;
-  if (total == 0) return 0;
-  upsample_add_fwd_kernel<<<blocks_for(total, 256), 256, 0, cudaStream_t(stream)>>>(x, a, out, per_image, Hi, Wi, Ho,
-                                                                                     Wo, C, total);
-  msda_b200_count_launches(1);
-  return int(cudaGetLastError());
+  if (N < 0 || per_image <= 0 || N % per_image != 0 || !up_shape_ok(Hi, Wi, Ho, Wo, C)) return TFB200_E_SHAPE;
+  return launch_up_fwd(x, a, out, UniformRows{per_image}, N, Hi, Wi, Ho, Wo, C, cudaStream_t(stream));
 }
 
 extern "C" int tfb200_upsample_add_bwd_f32(const float* dout, float* dx, float* da, int N, int per_image, int Hi,
                                            int Wi, int Ho, int Wo, int C, void* stream) {
   if (!dout || !dx || !da) return TFB200_E_NULLPTR;
-  if (N < 0 || per_image <= 0 || N % per_image != 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || C <= 0)
-    return TFB200_E_SHAPE;
-  if (N == 0) return 0;
-  const cudaStream_t s = cudaStream_t(stream);
-  const int64_t total = int64_t(N) * Hi * Wi * C, inner = int64_t(Ho) * Wo * C;
-  upsample_add_bwd_dx_kernel<<<blocks_for(total, 256), 256, 0, s>>>(dout, dx, Hi, Wi, Ho, Wo, C, total);
-  sum_queries_kernel<<<dim3(blocks_for(inner, 256), N / per_image), 256, 0, s>>>(dout, da, per_image, inner);
-  msda_b200_count_launches(2);
-  return int(cudaGetLastError());
+  if (N < 0 || per_image <= 0 || N % per_image != 0 || !up_shape_ok(Hi, Wi, Ho, Wo, C)) return TFB200_E_SHAPE;
+  return launch_up_bwd(dout, dx, da, UniformRows{per_image}, N / per_image, N, Hi, Wi, Ho, Wo, C,
+                       cudaStream_t(stream));
+}
+
+extern "C" int tfb200_upsample_add_rows_fwd_f32(const float* x, const float* a, const int32_t* row_offsets, float* out,
+                                                int B, int P, int Hi, int Wi, int Ho, int Wo, int C, void* stream) {
+  if (!row_offsets || (P > 0 && (!x || !out)) || (B > 0 && !a)) return TFB200_E_NULLPTR;
+  if (!rows_ok(B, P) || !up_shape_ok(Hi, Wi, Ho, Wo, C)) return TFB200_E_SHAPE;
+  return launch_up_fwd(x, a, out, RaggedRows{row_offsets, B}, P, Hi, Wi, Ho, Wo, C, cudaStream_t(stream));
+}
+
+extern "C" int tfb200_upsample_add_rows_bwd_f32(const float* dout, const int32_t* row_offsets, float* dx, float* da,
+                                                int B, int P, int Hi, int Wi, int Ho, int Wo, int C, void* stream) {
+  if (!row_offsets || (P > 0 && (!dout || !dx)) || (B > 0 && !da)) return TFB200_E_NULLPTR;
+  if (!rows_ok(B, P) || !up_shape_ok(Hi, Wi, Ho, Wo, C)) return TFB200_E_SHAPE;
+  return launch_up_bwd(dout, dx, da, RaggedRows{row_offsets, B}, B, P, Hi, Wi, Ho, Wo, C, cudaStream_t(stream));
 }
 
 extern "C" int tfb200_mask_loss_partial_chunks(int Ht, int Wt) {

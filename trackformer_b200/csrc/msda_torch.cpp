@@ -1154,6 +1154,154 @@ std::vector<at::Tensor> upsample_add_backward(const at::Tensor& dout, int64_t im
   return {dx, da};
 }
 
+// ---- ragged rows: P query rows over B images, image b owning rows offsets[b] .. offsets[b + 1] ----
+static const int32_t* check_offsets(const at::Tensor& offsets, const at::Tensor& like, int64_t B) {
+  TORCH_CHECK(offsets.is_cuda() && offsets.device() == like.device() && offsets.scalar_type() == at::kInt &&
+              offsets.dim() == 1 && offsets.numel() == B + 1 && offsets.is_contiguous(),
+              "row_offsets must be a contiguous int32 [B + 1] tensor on the device of the operands");
+  return offsets.data_ptr<int32_t>();
+}
+
+template <class T>
+static T* ptr_or_null(const at::Tensor& t) { return t.numel() > 0 ? t.data_ptr<T>() : nullptr; }
+
+// q [P, heads*32], k [B, HW, heads*32], pad [B, HW] bool or None, offsets int32 [B + 1] -> w [P, heads, HW]
+at::Tensor mask_attn_rows_forward(const at::Tensor& q, const at::Tensor& k, const c10::optional<at::Tensor>& pad,
+                                  const at::Tensor& offsets, int64_t heads, double scale) {
+  check_f32(q, "mask_attn_rows q");
+  check_f32(k, "mask_attn_rows k");
+  TORCH_CHECK(q.dim() == 2 && k.dim() == 3 && heads > 0 && q.size(1) == heads * 32 && k.size(2) == q.size(1) &&
+              k.size(1) > 0 && q.device() == k.device(), "mask_attn_rows: q [P, heads*32], k [B, HW, heads*32]");
+  const at::Tensor qc = q.contiguous(), kc = k.contiguous();
+  const int B = int(k.size(0)), P = int(q.size(0)), HW = int(k.size(1));
+  const int32_t* op = check_offsets(offsets, q, B);
+  const uint8_t* pp = nullptr;
+  at::Tensor pc;
+  if (pad.has_value() && pad->defined()) {
+    pc = pad->contiguous();
+    TORCH_CHECK(pc.is_cuda() && pc.element_size() == 1 && pc.numel() == int64_t(B) * HW,
+                "mask_attn_rows: pad must be a bool [B, HW] CUDA tensor");
+    pp = pc.numel() > 0 ? reinterpret_cast<const uint8_t*>(pc.data_ptr()) : nullptr;
+  }
+  const c10::cuda::CUDAGuard guard(q.device());
+  at::Tensor w = at::empty({P, heads, HW}, qc.options());
+  raise_rc(tfb200_mask_attn_rows_fwd_f32(ptr_or_null<float>(qc), ptr_or_null<float>(kc), pp, op, ptr_or_null<float>(w),
+                                         B, P, HW, int(heads), float(scale), c10::cuda::getCurrentCUDAStream().stream()),
+           "mask_attn_rows_forward");
+  return w;
+}
+
+std::vector<at::Tensor> mask_attn_rows_backward(const at::Tensor& q, const at::Tensor& k, const at::Tensor& offsets,
+                                                const at::Tensor& w, const at::Tensor& dw, double scale) {
+  check_f32(dw, "mask_attn_rows dw");
+  TORCH_CHECK(w.dim() == 3 && dw.sizes() == w.sizes() && q.dim() == 2 && q.size(0) == w.size(0) && k.dim() == 3 &&
+              q.is_contiguous() && k.is_contiguous() && w.is_contiguous(),
+              "mask_attn_rows_backward: saved tensors and dw [P, heads, HW]");
+  const int B = int(k.size(0)), P = int(w.size(0)), heads = int(w.size(1)), HW = int(w.size(2));
+  const int32_t* op = check_offsets(offsets, k, B);
+  const at::Tensor dwc = dw.contiguous();
+  const c10::cuda::CUDAGuard guard(k.device());
+  at::Tensor ds = at::empty_like(w), dq = at::empty_like(q), dk = at::empty_like(k);
+  raise_rc(tfb200_mask_attn_rows_bwd_f32(ptr_or_null<float>(q), ptr_or_null<float>(k), op, ptr_or_null<float>(w),
+                                         ptr_or_null<float>(dwc), ptr_or_null<float>(ds), ptr_or_null<float>(dq),
+                                         ptr_or_null<float>(dk), B, P, HW, heads, float(scale),
+                                         c10::cuda::getCurrentCUDAStream().stream()),
+           "mask_attn_rows_backward");
+  return {dq, dk};
+}
+
+static void check_rows_addend(const at::Tensor& addend, const at::Tensor& x) {
+  check_nhwc(addend, "group_norm_relu_rows addend");
+  TORCH_CHECK(addend.size(1) == x.size(1) && addend.size(2) == x.size(2) && addend.size(3) == x.size(3) &&
+              addend.device() == x.device(), "group_norm_relu_rows: addend must be [B, C, H, W] beside x [P, C, H, W]");
+}
+
+// x [P, C, H, W] + addend [B, C, H, W] broadcast over each image's rows -> {y, mean [P, G], rstd [P, G]}
+std::vector<at::Tensor> group_norm_relu_rows_forward(const at::Tensor& x, const at::Tensor& addend,
+                                                     const at::Tensor& offsets, const at::Tensor& gamma,
+                                                     const at::Tensor& beta, int64_t groups, double eps) {
+  check_nhwc(x, "group_norm_relu_rows x");
+  check_rows_addend(addend, x);
+  const int64_t C = x.size(1), B = addend.size(0);
+  check_f32(gamma, "group_norm_relu_rows gamma");
+  check_f32(beta, "group_norm_relu_rows beta");
+  TORCH_CHECK(gamma.numel() == C && beta.numel() == C && gamma.is_contiguous() && beta.is_contiguous(),
+              "group_norm_relu_rows: gamma / beta [C]");
+  const int32_t* op = check_offsets(offsets, x, B);
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor y = empty_nhwc(x.sizes(), x);
+  at::Tensor mean = at::empty({x.size(0), groups}, x.options()), rstd = at::empty({x.size(0), groups}, x.options());
+  raise_rc(tfb200_group_norm_relu_rows_fwd_f32(ptr_or_null<float>(x), ptr_or_null<float>(addend), op,
+                                               gamma.data_ptr<float>(), beta.data_ptr<float>(), ptr_or_null<float>(y),
+                                               ptr_or_null<float>(mean), ptr_or_null<float>(rstd), int(B),
+                                               int(x.size(0)), x.size(2) * x.size(3), int(C), int(groups), float(eps),
+                                               c10::cuda::getCurrentCUDAStream().stream()),
+           "group_norm_relu_rows_forward");
+  return {y, mean, rstd};
+}
+
+// -> {dx, daddend [B, C, H, W], dgamma, dbeta}
+std::vector<at::Tensor> group_norm_relu_rows_backward(const at::Tensor& dy, const at::Tensor& x,
+                                                      const at::Tensor& addend, const at::Tensor& offsets,
+                                                      const at::Tensor& y, const at::Tensor& gamma,
+                                                      const at::Tensor& mean, const at::Tensor& rstd) {
+  check_nhwc(x, "group_norm_relu_rows x");
+  check_nhwc(y, "group_norm_relu_rows y");
+  check_f32(dy, "group_norm_relu_rows dy");
+  check_rows_addend(addend, x);
+  TORCH_CHECK(dy.sizes() == x.sizes() && y.sizes() == x.sizes() && mean.dim() == 2 && mean.size(0) == x.size(0),
+              "group_norm_relu_rows_backward: dy, x, y must have one shape");
+  const at::Tensor dyc = dy.contiguous(at::MemoryFormat::ChannelsLast);
+  const int64_t P = x.size(0), C = x.size(1), B = addend.size(0);
+  const int32_t* op = check_offsets(offsets, x, B);
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor dx = empty_nhwc(x.sizes(), x), da = empty_nhwc(addend.sizes(), x);
+  at::Tensor daff = at::empty({2, C}, x.options()), ws = at::empty({P, 2, C}, x.options());
+  raise_rc(tfb200_group_norm_relu_rows_bwd_f32(ptr_or_null<float>(dyc), ptr_or_null<float>(x),
+                                               ptr_or_null<float>(addend), op, ptr_or_null<float>(y),
+                                               gamma.data_ptr<float>(), ptr_or_null<float>(mean),
+                                               ptr_or_null<float>(rstd), ptr_or_null<float>(dx), ptr_or_null<float>(da),
+                                               daff.data_ptr<float>(), ptr_or_null<float>(ws), int(B), int(P),
+                                               x.size(2) * x.size(3), int(C), int(mean.size(1)),
+                                               c10::cuda::getCurrentCUDAStream().stream()),
+           "group_norm_relu_rows_backward");
+  return {dx, da, daff[0], daff[1]};
+}
+
+// a [B, C, Ho, Wo] (broadcast over each image's rows) + nearest_upsample(x [P, C, Hi, Wi]), both channels-last
+at::Tensor upsample_add_rows_forward(const at::Tensor& x, const at::Tensor& a, const at::Tensor& offsets) {
+  check_nhwc(x, "upsample_add_rows x");
+  check_nhwc(a, "upsample_add_rows a");
+  TORCH_CHECK(a.size(1) == x.size(1) && a.device() == x.device(),
+              "upsample_add_rows: x [P, C, Hi, Wi] and a [B, C, Ho, Wo]");
+  const int32_t* op = check_offsets(offsets, x, a.size(0));
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor out = empty_nhwc({x.size(0), x.size(1), a.size(2), a.size(3)}, x);
+  raise_rc(tfb200_upsample_add_rows_fwd_f32(ptr_or_null<float>(x), ptr_or_null<float>(a), op, ptr_or_null<float>(out),
+                                            int(a.size(0)), int(x.size(0)), int(x.size(2)), int(x.size(3)),
+                                            int(a.size(2)), int(a.size(3)), int(x.size(1)),
+                                            c10::cuda::getCurrentCUDAStream().stream()),
+           "upsample_add_rows_forward");
+  return out;
+}
+
+std::vector<at::Tensor> upsample_add_rows_backward(const at::Tensor& dout, const at::Tensor& offsets, int64_t Hi,
+                                                   int64_t Wi) {
+  check_f32(dout, "upsample_add_rows dout");
+  TORCH_CHECK(dout.dim() == 4 && Hi > 0 && Wi > 0, "upsample_add_rows_backward: dout [P, C, Ho, Wo]");
+  const at::Tensor g = dout.contiguous(at::MemoryFormat::ChannelsLast);
+  const int64_t P = g.size(0), C = g.size(1), B = offsets.numel() - 1;
+  TORCH_CHECK(B >= 0, "upsample_add_rows_backward: row_offsets must have B + 1 entries");
+  const int32_t* op = check_offsets(offsets, g, B);
+  const c10::cuda::CUDAGuard guard(g.device());
+  at::Tensor dx = empty_nhwc({P, C, Hi, Wi}, g), da = empty_nhwc({B, C, g.size(2), g.size(3)}, g);
+  raise_rc(tfb200_upsample_add_rows_bwd_f32(ptr_or_null<float>(g), op, ptr_or_null<float>(dx), ptr_or_null<float>(da),
+                                            int(B), int(P), int(Hi), int(Wi), int(g.size(2)), int(g.size(3)), int(C),
+                                            c10::cuda::getCurrentCUDAStream().stream()),
+           "upsample_add_rows_backward");
+  return {dx, da};
+}
+
 static void check_mask_loss_args(const at::Tensor& logits, const at::Tensor& src, const at::Tensor& tgt_masks,
                                  const at::Tensor& tgt, const at::Tensor& num_boxes) {
   check_f32(logits, "mask_loss logits");
@@ -1295,6 +1443,12 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("group_norm_relu_backward", &group_norm_relu_backward);
   m.def("upsample_add_forward", &upsample_add_forward);
   m.def("upsample_add_backward", &upsample_add_backward);
+  m.def("mask_attn_rows_forward", &mask_attn_rows_forward);
+  m.def("mask_attn_rows_backward", &mask_attn_rows_backward);
+  m.def("group_norm_relu_rows_forward", &group_norm_relu_rows_forward);
+  m.def("group_norm_relu_rows_backward", &group_norm_relu_rows_backward);
+  m.def("upsample_add_rows_forward", &upsample_add_rows_forward);
+  m.def("upsample_add_rows_backward", &upsample_add_rows_backward);
   m.def("mask_loss_forward", &mask_loss_forward);
   m.def("mask_loss_backward", &mask_loss_backward);
   m.def("track_masks", &track_masks);

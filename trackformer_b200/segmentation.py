@@ -78,6 +78,71 @@ class _UpsampleAdd(Function):
         return dx, da
 
 
+class _MaskAttnRows(Function):
+    @staticmethod
+    def forward(ctx, q, k, pad, offsets, heads, scale):
+        w = ext.load().mask_attn_rows_forward(q, k, pad, offsets, heads, scale)
+        ctx.save_for_backward(q.contiguous(), k.contiguous(), offsets, w)
+        ctx.scale = scale
+        return w
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dw):
+        q, k, offsets, w = ctx.saved_tensors
+        dq, dk = ext.load().mask_attn_rows_backward(q, k, offsets, w, dw, ctx.scale)
+        return dq, dk, None, None, None, None
+
+
+class _GroupNormReLURows(Function):
+    @staticmethod
+    def forward(ctx, x, addend, offsets, gamma, beta, groups, eps):
+        y, mean, rstd = ext.load().group_norm_relu_rows_forward(x, addend, offsets, gamma, beta, groups, eps)
+        ctx.save_for_backward(x, addend, offsets, y, gamma, mean, rstd)
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        x, addend, offsets, y, gamma, mean, rstd = ctx.saved_tensors
+        dx, da, dgamma, dbeta = ext.load().group_norm_relu_rows_backward(dy, x, addend, offsets, y, gamma, mean, rstd)
+        return dx, da, None, dgamma, dbeta, None, None
+
+
+class _UpsampleAddRows(Function):
+    @staticmethod
+    def forward(ctx, x, a, offsets):
+        ctx.save_for_backward(offsets)
+        ctx.geom = (x.shape[2], x.shape[3])
+        return ext.load().upsample_add_rows_forward(x, a, offsets)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        offsets, = ctx.saved_tensors
+        dx, da = ext.load().upsample_add_rows_backward(dout, offsets, *ctx.geom)
+        return dx, da, None
+
+
+class RaggedRows:
+    """Query rows owned unevenly by the images of a batch: image b owns rows ``offsets[b] .. offsets[b + 1]``.
+    ``offsets`` int32 [B + 1] and ``image`` int64 [P] (row -> image) live on the device; ``sizes`` are the host counts
+    they were built from, so nothing is read back."""
+
+    def __init__(self, sizes, device):
+        self.sizes = [int(n) for n in sizes]
+        acc = [0]
+        for n in self.sizes:
+            acc.append(acc[-1] + n)
+        self.offsets = torch.tensor(acc, dtype=torch.int32).to(device, non_blocking=True)
+        self.image = torch.repeat_interleave(torch.arange(len(self.sizes)),
+                                             torch.tensor(self.sizes, dtype=torch.long)).to(device, non_blocking=True)
+
+    @property
+    def total(self) -> int:
+        return sum(self.sizes)
+
+
 def group_norm_relu(x: Tensor, gn: nn.GroupNorm, addend: Optional[Tensor] = None, per_image: int = 1) -> Tensor:
     """``relu(gn(x + addend[n // per_image]))`` on channels-last CUDA fp32 maps (csrc/mask_head.cu)."""
     cl = torch.channels_last
@@ -138,10 +203,22 @@ class MaskHeadSmallConv(nn.Module):
         return ((self.adapter1, self.lay3, self.gn3), (self.adapter2, self.lay4, self.gn4),
                 (self.adapter3, self.lay5, self.gn5))
 
-    def forward(self, x: Tensor, bbox_mask: Tensor, fpns: List[Tensor]):
-        """x [B, C, H, W] per image, bbox_mask [B, Q, heads, H, W], fpns per image -> [B * Q, 1, H4, W4]"""
+    def forward(self, x: Tensor, bbox_mask: Tensor, fpns: List[Tensor], rows: Optional[RaggedRows] = None):
+        """x [B, C, H, W] per image, bbox_mask [B, Q, heads, H, W], fpns per image -> [B * Q, 1, H4, W4].
+        With ``rows``: bbox_mask [P, heads, H, W], row p belonging to image ``rows.image[p]`` -> [P, 1, H4, W4]."""
         if x.is_cuda and x.dtype == torch.float32:
+            if rows is not None:
+                return self._forward_cuda_rows(x, bbox_mask, fpns, rows)
             return self._forward_cuda(x, bbox_mask, fpns)
+        if rows is not None:
+            x = torch.cat([x.index_select(0, rows.image), bbox_mask], 1)
+            x = F.relu(self.gn1(self.lay1(x)))
+            x = F.relu(self.gn2(self.lay2(x)))
+            for (adapter, lay, gn), fpn in zip(self._stages(), fpns):
+                cur_fpn = adapter(fpn).index_select(0, rows.image)
+                x = cur_fpn + F.interpolate(x, size=cur_fpn.shape[-2:], mode="nearest")
+                x = F.relu(gn(lay(x)))
+            return self.out_lay(x)
         x = torch.cat([_expand(x, bbox_mask.shape[1]), bbox_mask.flatten(0, 1)], 1)
         x = F.relu(self.gn1(self.lay1(x)))
         x = F.relu(self.gn2(self.lay2(x)))
@@ -167,6 +244,23 @@ class MaskHeadSmallConv(nn.Module):
             y = group_norm_relu(lay(y), gn)
         return self.out_lay(y)
 
+    def _forward_cuda_rows(self, x, bbox_mask, fpns, rows):
+        """``_forward_cuda`` over ragged rows: the per-image terms enter the ragged kernels, which broadcast them over
+        each image's rows and sum their gradients over those rows."""
+        cl = torch.channels_last
+        n_src = x.shape[1]
+        per_image = F.conv2d(x.contiguous(memory_format=cl), self.lay1.weight[:, :n_src], self.lay1.bias, padding=1)
+        y = F.conv2d(bbox_mask.contiguous(memory_format=cl), self.lay1.weight[:, n_src:], None, padding=1)
+        y = _GroupNormReLURows.apply(y.contiguous(memory_format=cl), per_image.contiguous(memory_format=cl),
+                                     rows.offsets, self.gn1.weight, self.gn1.bias, self.gn1.num_groups,
+                                     float(self.gn1.eps))
+        y = group_norm_relu(self.lay2(y), self.gn2)
+        for (adapter, lay, gn), fpn in zip(self._stages(), fpns):
+            a = adapter(fpn.contiguous(memory_format=cl)).contiguous(memory_format=cl)
+            y = _UpsampleAddRows.apply(y.contiguous(memory_format=cl), a, rows.offsets)
+            y = group_norm_relu(lay(y), gn)
+        return self.out_lay(y)
+
 
 class MHAttentionMap(nn.Module):
     """Attention softmax of the queries over a 2-d map, without the value product (detr_segmentation.py:200-216)."""
@@ -186,8 +280,11 @@ class MHAttentionMap(nn.Module):
         nn.init.xavier_uniform_(self.q_linear.weight)
         self.normalize_fact = float(hidden_dim / self.num_heads) ** -0.5
 
-    def forward(self, q, k, mask: Optional[Tensor] = None):
-        """q [B, Q, D], k [B, D, H, W] (may be a view of token-major memory), mask [B, H, W] -> [B, Q, heads, H, W]"""
+    def forward(self, q, k, mask: Optional[Tensor] = None, rows: Optional[RaggedRows] = None):
+        """q [B, Q, D], k [B, D, H, W] (may be a view of token-major memory), mask [B, H, W] -> [B, Q, heads, H, W].
+        With ``rows``: q [P, D], row p attending to image ``rows.image[p]`` -> [P, heads, H, W]."""
+        if rows is not None:
+            return self._forward_rows(q, k, mask, rows)
         if q.is_cuda and q.dtype == torch.float32:
             b, _, h, w = k.shape
             k_tok = k.permute(0, 2, 3, 1).reshape(b, h * w, k.shape[1])     # a view of token-major encoder memory
@@ -204,6 +301,25 @@ class MHAttentionMap(nn.Module):
         if mask is not None:
             weights.masked_fill_(mask.unsqueeze(1).unsqueeze(1), float("-inf"))
         weights = F.softmax(weights.flatten(2), dim=-1).view_as(weights)
+        return self.dropout(weights)
+
+    def _forward_rows(self, q, k, mask, rows):
+        b, _, h, w = k.shape
+        if q.is_cuda and q.dtype == torch.float32:
+            k_tok = k.permute(0, 2, 3, 1).reshape(b, h * w, k.shape[1])
+            qp = fused_linear(q, self.q_linear.weight, self.q_linear.bias).contiguous()
+            kp = fused_linear(k_tok, self.k_linear.weight, self.k_linear.bias).contiguous()
+            pad = None if mask is None else mask.reshape(b, h * w)
+            weights = _MaskAttnRows.apply(qp, kp, pad, rows.offsets, self.num_heads, self.normalize_fact)
+            return self.dropout(weights.view(q.shape[0], self.num_heads, h, w))
+        q = self.q_linear(q)
+        k = F.conv2d(k, self.k_linear.weight.unsqueeze(-1).unsqueeze(-1), self.k_linear.bias)
+        qh = q.view(q.shape[0], self.num_heads, self.hidden_dim // self.num_heads)
+        kh = k.view(b, self.num_heads, self.hidden_dim // self.num_heads, h, w).index_select(0, rows.image)
+        weights = torch.einsum("pnc,pnchw->pnhw", qh * self.normalize_fact, kh)
+        if mask is not None:
+            weights = weights.masked_fill(mask.index_select(0, rows.image).unsqueeze(1), float("-inf"))
+        weights = F.softmax(weights.flatten(1), dim=-1).view_as(weights)
         return self.dropout(weights)
 
 
@@ -231,7 +347,18 @@ class DETRSegmBase(nn.Module):
     def mask_logits(self, features, memory, hs, rows=None) -> Tensor:
         """Mask logits ``[B, len(rows), H/4, W/4]`` of the query rows ``rows`` (all rows if None) from the outputs of
         ``detect``.  Every query has its own attention softmax and its own GroupNorm sample, so a row's logits do not
-        depend on which other rows are computed with it."""
+        depend on which other rows are computed with it.
+
+        ``rows=(src, sizes)`` selects a different set of rows per image: image b contributes ``sizes[b]`` rows (host
+        ints), ``src`` [sum(sizes)] (device) holds their query indices image after image.  The result is then the
+        compact ``[sum(sizes), H/4, W/4]``: row i is the mask of query ``src[i]`` of its image (a training step's
+        matched queries; nothing is read back from the device)."""
+        return self.mask_logits_from(*self.mask_inputs(features, memory, hs), rows=rows)
+
+    def mask_inputs(self, features, memory, hs):
+        """What the mask branch reads from the detector: ``(queries [B, Q, D], memory map [B, D, h, w], src map
+        [B, D, h, w], its pad mask [B, h, w], fpns)`` -- the last decoder layer, the attention keys, the per-image
+        ``lay1`` input and the three FPN maps, for the deformable and the vanilla layout."""
         if isinstance(memory, list):                               # deformable: per-level memory, stride 16 (layer3)
             src, mask = features[-2].decompose()
             src = self.input_proj[-3](src)
@@ -243,9 +370,22 @@ class DETRSegmBase(nn.Module):
             src, mask = features[-1].decompose()
             src = self.input_proj(src)
             fpns = [features[2].tensors, features[1].tensors, features[0].tensors]
-        batch_size = src.shape[0]
+        return hs[-1], memory, src, mask, fpns
 
-        q = hs[-1]
+    def mask_logits_from(self, q, memory, src, mask, fpns, rows=None) -> Tensor:
+        """``mask_logits`` from the outputs of ``mask_inputs``."""
+        batch_size = src.shape[0]
+        if isinstance(rows, tuple):
+            src_rows, sizes = rows
+            ragged = RaggedRows(sizes, q.device)
+            if ragged.total == 0:
+                h4, w4 = fpns[-1].shape[-2:]
+                return q.new_zeros((0, h4, w4))
+            flat = ragged.image * q.shape[1] + src_rows.to(device=q.device, dtype=torch.long)
+            q = q.flatten(0, 1).index_select(0, flat)
+            bbox_mask = self.bbox_attention(q, memory, mask=mask, rows=ragged)
+            seg_masks = self.mask_head(src, bbox_mask, fpns, rows=ragged)
+            return seg_masks.view(ragged.total, seg_masks.shape[-2], seg_masks.shape[-1])
         if rows is not None:
             q = q.index_select(1, torch.as_tensor(rows, dtype=torch.long, device=q.device))
         bbox_mask = self.bbox_attention(q, memory, mask=mask)

@@ -36,15 +36,27 @@ from torch import nn
 
 
 class _DetectorCore(nn.Module):
-    """Tensor-in / tensors-out view of the detector for graph capture: frames -> (logits[K,B,Q,C], boxes[K,B,Q,4])."""
+    """Tensor-in / tensors-out view of the detector for graph capture: frames -> (logits[K,B,Q,C], boxes[K,B,Q,4]).
 
-    def __init__(self, model):
+    With ``masks`` (segmentation models) the detector runs without its mask head and the mask branch's inputs
+    follow the two heads: ``(logits, boxes, queries, memory, src, pad, fpn0, fpn1, fpn2)`` (``DETRSegmBase.mask_inputs``);
+    the step runs the head itself on the matched rows only."""
+
+    def __init__(self, model, masks: bool = False):
         super().__init__()
         self.model = model
+        self.masks = masks
 
     def forward(self, frames):
+        if self.masks:
+            out, _, features, memory, hs = self.model.detect(frames, None, None)
+            return self._heads(out) + self._mask_inputs(features, memory, hs)
         out, _, _, _, _ = self.model(frames, None, None)
         return self._heads(out)
+
+    def _mask_inputs(self, features, memory, hs):
+        q, memory, src, pad, fpns = self.model.mask_inputs(features, memory, hs)
+        return (q, memory, src, pad, *fpns)
 
     def detector(self, frames, targets=None, prev_features=None):
         """The detector's own forward (``DeformableDETR.forward``) of a tracking model: previous frames, and current
@@ -53,13 +65,15 @@ class _DetectorCore(nn.Module):
         return super(DETRTrackingBase, self.model).forward(frames, targets, prev_features)
 
     def track(self, frames, targets, prev_features):
-        out, _, _, _, _ = self.detector(frames, targets, prev_features)
+        out, _, features, memory, hs = self.detector(frames, targets, prev_features)
+        if self.masks:
+            return self._heads(out) + self._mask_inputs(features, memory, hs)
         return self._heads(out)
 
     def _heads(self, out):
         stacked = getattr(self.model, "stacked_heads", None)
         if stacked is not None and stacked[0].shape[0] == len(out["aux_outputs"]) + 1:
-            return stacked                           # the very tensors the dictionary entries are slices of
+            return tuple(stacked)                    # the very tensors the dictionary entries are slices of
         logits = torch.stack([a["pred_logits"] for a in out["aux_outputs"]] + [out["pred_logits"]])
         boxes = torch.stack([a["pred_boxes"] for a in out["aux_outputs"]] + [out["pred_boxes"]])
         return logits, boxes
@@ -70,19 +84,30 @@ class TrainStep:
 
     def __init__(self, model, criterion, optimizer_factory=None, max_norm: float = 0.1,
                  use_graphs: bool = True, example_frames: Optional[torch.Tensor] = None,
-                 example_targets: Optional[list] = None, flat_adamw: Optional[dict] = None, track_bucket: int = 32):
+                 example_targets: Optional[list] = None, flat_adamw: Optional[dict] = None, track_bucket: int = 32,
+                 masks: bool = False):
         """``optimizer_factory(params)`` builds any torch optimizer; ``flat_adamw={'groups': [...], 'betas':..., 'eps':...}``
         (groups as for torch.optim.AdamW, e.g. flat_adamw.reference_param_groups(model)) instead lays the PARAMETERS out
         flat as well and updates them with the one-pass clip + AdamW kernel.  ``track_bucket``: tracking steps pad their
-        track queries up to a multiple of it, and one pair of current-frame graphs is captured per padded count."""
+        track queries up to a multiple of it, and one pair of current-frame graphs is captured per padded count.
+
+        ``masks=True`` trains a segmentation model (``DETRSegmBase``, with ``freeze_detr`` or without) with a criterion
+        whose losses are ``labels`` / ``boxes`` / ``cardinality`` / ``masks``: the graphs end at the mask head's inputs,
+        and between them the mask head runs eagerly on the last layer's matched query rows only (see ``_mask_loss``)."""
         if track_bucket < 1:
             raise ValueError("track_bucket must be >= 1")
         self.track_bucket = int(track_bucket)
         self._prev_plans, self._track_plans = {}, {}
         self.track_captures = 0
-        if hasattr(model, "mask_head") or "masks" in getattr(criterion, "losses", ()):
-            raise NotImplementedError("TrainStep does not train segmentation models (their mask losses would be "
-                                      "dropped); run the model and SetCriterion eagerly instead")
+        segm = hasattr(model, "mask_head") or "masks" in getattr(criterion, "losses", ())
+        if segm and not masks:
+            raise NotImplementedError("TrainStep trains segmentation models only with masks=True (without it their "
+                                      "mask losses would be dropped); or run the model and SetCriterion eagerly")
+        if masks and not (hasattr(model, "mask_head") and hasattr(model, "mask_inputs")
+                          and set(getattr(criterion, "losses", ())) == {"labels", "boxes", "cardinality", "masks"}):
+            raise ValueError("masks=True needs a segmentation model and a criterion with the losses labels, boxes, "
+                             "cardinality and masks")
+        self.masks = bool(masks)
         self.model = model
         self.criterion = criterion
         self.max_norm = max_norm
@@ -91,7 +116,7 @@ class TrainStep:
         if prepare is not None:
             prepare()                                   # final parameter memory formats before gradient views exist
         self.params: List[nn.Parameter] = [p for p in model.parameters() if p.requires_grad]
-        self.core = _DetectorCore(model)
+        self.core = _DetectorCore(model, self.masks)
         # The loss normaliser (world-averaged box count, detr.py:397-401) is a device scalar in a static buffer, refreshed
         # every step by ONE scalar all-reduce that every rank issues on every path -- so ranks may take different
         # paths (full-step graph / two graphs / eager) in the same step and still run the same collective sequence.
@@ -140,7 +165,9 @@ class TrainStep:
         trunk = getattr(getattr(model, "backbone", [None])[0], "body", None)
         contiguous_tail = all(is_bb(p) for p in self.params[i_bb:]) and \
             all(".layer4." in names[id(p)] for p in self.params[i_l4:])
-        self.phased = (self.world > 1 and os.environ.get("TFB200_OVERLAP_AR", "1") != "0" and trunk is not None
+        # (not for mask models: their single flat all-reduce follows the eager mask branch, same order on every rank)
+        self.phased = (self.world > 1 and not self.masks and os.environ.get("TFB200_OVERLAP_AR", "1") != "0"
+                       and trunk is not None
                        and hasattr(trunk, "cut") and 0 < i_bb < i_l4 < len(self.params) and contiguous_tail)
         self._trunk, self._i_bb, self._i_l4 = trunk, i_bb, i_l4
         off_bb = offsets[i_bb] if i_bb < len(offsets) else total
@@ -160,6 +187,9 @@ class TrainStep:
         for p, o in zip(self.params, offsets):
             p.grad = flat_view(self.flat_grad, p, o)
         self._views = [p.grad for p in self.params]
+        head = ("mask_head.", "bbox_attention.")
+        self._mask_params = [p for p in self.params if names.get(id(p), "").startswith(head)]
+        self._mask_views = [p.grad for p in self._mask_params]
         self.flat_param = None
         self.flat_optimizer = None
         if groups is not None:
@@ -175,8 +205,11 @@ class TrainStep:
         self.optimizer = optimizer_factory(self.params) if optimizer_factory is not None else None
         if use_graphs:
             assert example_frames is not None and example_frames.is_cuda
-            self._capture(example_frames)
-            if example_targets is not None and getattr(criterion, "device_matcher", False):
+            if self.masks:
+                self._capture_masks(example_frames)
+            else:
+                self._capture(example_frames)
+            if example_targets is not None and getattr(criterion, "device_matcher", False) and not self.masks:
                 self._capture_full(example_targets)
 
     # ------------------------------------------------------------------------------------------
@@ -204,6 +237,14 @@ class TrainStep:
             self.flat_grad.zero_()
             torch.autograd.backward((self.s_logits, self.s_boxes), (self.s_glogits, self.s_gboxes))
         self.flat_grad.zero_()
+
+    def _capture_masks(self, example: torch.Tensor) -> None:
+        """``_capture`` for a segmentation model: the forward graph ends at the heads and the mask branch's inputs, the
+        backward graph takes a cotangent for each of them that requires grad (none with ``freeze_detr``: no graph)."""
+        self.static_frames = example.clone()
+        self._pool = torch.cuda.graph_pool_handle()
+        self.g_fwd, self.s_outs, self.g_bwd, self.s_grads = self._warm_up_and_capture(
+            lambda: self.core(self.static_frames), backward=True, count=False)
 
     def _capture_full(self, example_targets: list) -> None:
         """ONE graph for forward + matching cost + device Hungarian matching + loss + backward, usable whenever the
@@ -365,12 +406,17 @@ class TrainStep:
             if g is None:
                 v.zero_()
 
-    def _loss(self, logits, boxes, targets, num_boxes=None, track_queries=False):
-        """Weighted total of the criterion's entries (engine.py:139-140: sum(loss_dict[k] * weight_dict[k]))."""
+    def _loss(self, logits, boxes, targets, num_boxes=None, track_queries=False, with_dict=False):
+        """Weighted total of the criterion's entries (engine.py:139-140: sum(loss_dict[k] * weight_dict[k]));
+        ``with_dict``: -> (total, loss dictionary)."""
         if track_queries:
             loss_dict = self.criterion.forward_stacked(logits, boxes, targets, num_boxes, track_queries=True)
         else:
             loss_dict = self.criterion.forward_stacked(logits, boxes, targets, num_boxes)
+        total = self._total(loss_dict)
+        return (total, loss_dict) if with_dict else total
+
+    def _total(self, loss_dict):
         wd = self.criterion.weight_dict
         stacked = getattr(loss_dict, "stacked", None)
         names = ("loss_ce", "loss_bbox", "loss_giou")
@@ -385,6 +431,60 @@ class TrainStep:
                 self._loss_w_key = key
             return (torch.stack(stacked) * self._loss_w).sum()
         return sum(loss_dict[k] * wd[k] for k in loss_dict if k in wd)
+
+    # ------------------------------------------------------------------------------------------ masks
+    def _mask_loss(self, outs, targets, num_boxes, track_queries):
+        """The whole weighted loss of a segmentation step from the detector's outputs ``outs`` (see ``_DetectorCore``).
+
+        The box, class and cardinality terms come from ``forward_stacked`` as for the box-only models; the mask head
+        then runs on the last layer's matched query rows only (``LossDict.matched``), image after image, and their
+        compact logits ``[P, h, w]`` are scored pair by pair.  The reference runs the head on every query and reads the
+        matched rows (detr.py:330-357): the rows are independent (own attention softmax, own GroupNorm sample, no
+        dropout), so the losses and gradients are the same and unmatched rows -- filler track queries included --
+        get zero gradient either way.  No host synchronisation: the per-image counts come from the targets."""
+        from .criterion import mask_losses
+        logits, boxes, q, memory, src, pad, *fpns = outs
+        box_loss, loss_dict = self._loss(logits, boxes, targets, num_boxes, track_queries, with_dict=True)
+        if num_boxes is None:
+            num_boxes = self.criterion._num_boxes(targets, logits.device)
+        _, rows, tgt = loss_dict.matched
+        if sum(loss_dict.matched_sizes) == 0:           # no pair: both mask losses are 0 (detr.py:330-357)
+            return box_loss
+        pred =self.model.mask_logits_from(q, memory, src, pad, fpns, rows=(rows, loss_dict.matched_sizes))
+        found = mask_losses(pred[None], torch.arange(pred.shape[0], device=pred.device), tgt, targets, num_boxes)
+        wd = self.criterion.weight_dict
+        return box_loss + found["loss_mask"] * wd["loss_mask"] + found["loss_dice"] * wd["loss_dice"]
+
+    def _mask_backward(self, loss) -> None:
+        """``_backward_into_flat`` of a segmentation step (eager paths)."""
+        if loss.requires_grad:
+            self._backward_into_flat(loss)
+        else:                                   # frozen detector and no matched row: nothing trains
+            self.flat_grad.zero_()
+
+    def _mask_step_replayed(self, outs, grads, g_bwd, targets, num_boxes, track_queries):
+        """A segmentation step between its graphs (``outs`` just replayed): loss, mask branch and ONE autograd.grad
+        into the cotangent buffers ``grads`` and the mask head's parameters, then the backward graph (which zero-fills
+        ``flat_grad``) and only after it the mask head's gradients into their slices of ``flat_grad``."""
+        leaves = [o.detach().requires_grad_(True) if g is not None else o.detach() for o, g in zip(outs, grads)]
+        loss = self._mask_loss(leaves, targets, num_boxes, track_queries)
+        inputs = [x for x, g in zip(leaves, grads) if g is not None]
+        wrt = inputs + self._mask_params
+        got = torch.autograd.grad(loss, wrt, allow_unused=True) if loss.requires_grad and wrt else [None] * len(wrt)
+        for dst, g in zip([g for g in grads if g is not None], got[:len(inputs)]):
+            if g is None:
+                dst.zero_()
+            else:
+                dst.copy_(g)
+        if g_bwd is not None:
+            g_bwd.replay()
+        else:
+            self.flat_grad.zero_()
+        head = got[len(inputs):]
+        dst = [v for v, g in zip(self._mask_views, head) if g is not None]
+        if dst:
+            torch._foreach_copy_(dst, [g for g in head if g is not None])
+        return loss
 
     # ------------------------------------------------------------------------------------------ tracking
     def _tracking_route(self, targets) -> str:
@@ -402,8 +502,9 @@ class TrainStep:
         if (not isinstance(model, DETRTrackingBase) or not model.training or model._tracking or not targets
                 or "prev_image" not in targets[0]):
             return "detect"
+        losses = {"labels", "boxes", "cardinality"} | ({"masks"} if getattr(self, "masks", False) else set())
         if ("prev_prev_image" in targets[0] or model._backprop_prev_frame
-                or set(crit.losses) != {"labels", "boxes", "cardinality"}
+                or set(crit.losses) != losses
                 or not hasattr(crit.matcher, "match_layers_forced")):
             return "eager"
         return "track"
@@ -419,18 +520,20 @@ class TrainStep:
     def _graphs(self) -> bool:
         return self.g_fwd is not None
 
-    def _warm_up_and_capture(self, run, backward: bool):
+    def _warm_up_and_capture(self, run, backward: bool, count: bool = True):
         """Capture ``run`` (and, with ``backward``, the zero-fill + backward of its outputs) into graphs of the step's
         pool.  The warm-up passes draw nothing from the CPU generator; its state is restored regardless, so that the
-        track-query decisions of a step do not depend on whether it captured."""
+        track-query decisions of a step do not depend on whether it captured.  Outputs that do not require grad get no
+        cotangent buffer (None in ``grads``); when none does, there is no backward graph."""
         with torch.random.fork_rng(devices=[]):
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
                 for _ in range(2):
                     outs = run()
-                    if backward:
-                        torch.autograd.backward(outs, [torch.zeros_like(o) for o in outs])
+                    diff = [o for o in outs if o.requires_grad]
+                    if backward and diff:
+                        torch.autograd.backward(diff, [torch.zeros_like(o) for o in diff])
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
             g_fwd = torch.cuda.CUDAGraph()
@@ -438,13 +541,16 @@ class TrainStep:
                 outs = run()
             g_bwd = grads = None
             if backward:
-                grads = [torch.zeros_like(o) for o in outs]
-                g_bwd = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g_bwd, pool=self._pool):
-                    self.flat_grad.zero_()
-                    torch.autograd.backward(outs, grads)
+                grads = [torch.zeros_like(o) if o.requires_grad else None for o in outs]
+                diff = [(o, g) for o, g in zip(outs, grads) if g is not None]
+                if diff:
+                    g_bwd = torch.cuda.CUDAGraph()
+                    with torch.cuda.graph(g_bwd, pool=self._pool):
+                        self.flat_grad.zero_()
+                        torch.autograd.backward([o for o, _ in diff], [g for _, g in diff])
                 self.flat_grad.zero_()
-        self.track_captures += 1
+        if count:
+            self.track_captures += 1
         return g_fwd, outs, g_bwd, grads
 
     def _previous_frame(self, targets):
@@ -559,6 +665,10 @@ class TrainStep:
             return self.core.track(plan["frames"], track_targets, prev_features)
 
         if not graphed:
+            if self.masks:
+                loss = self._mask_loss(run(), loss_targets, num_boxes, True)
+                self._mask_backward(loss)
+                return loss
             logits, boxes = run()
             loss = self._loss(logits, boxes, loss_targets, num_boxes, track_queries=True)
             self._backward_into_flat(loss)
@@ -566,6 +676,8 @@ class TrainStep:
         if new:
             plan["g_fwd"], plan["outs"], plan["g_bwd"], plan["grads"] = self._warm_up_and_capture(run, backward=True)
         plan["g_fwd"].replay()
+        if self.masks:
+            return self._mask_step_replayed(plan["outs"], plan["grads"], plan["g_bwd"], loss_targets, num_boxes, True)
         logits, boxes = (o.detach().requires_grad_(True) for o in plan["outs"])
         loss = self._loss(logits, boxes, loss_targets, num_boxes, track_queries=True)
         for dst, g in zip(plan["grads"], torch.autograd.grad(loss, (logits, boxes))):
@@ -618,7 +730,8 @@ class TrainStep:
         full = (route == "detect" and self.g_full is not None
                 and tuple(len(t["labels"]) for t in targets) == self.full_sizes)
         # one scalar all-reduce per step on EVERY path, before anything else (same collective order on all ranks)
-        num_boxes = self._normaliser(targets, dev) if (self.world > 1 or full or route == "track") else None
+        num_boxes = self._normaliser(targets, dev) if (self.world > 1 or full or route == "track"
+                                                       or self.masks) else None
         pending = None
         if route != "detect":
             loss = (self._track_step if route == "track" else self._tracking_eager)(frames, targets, num_boxes)
@@ -647,6 +760,18 @@ class TrainStep:
             pending.append(self._all_reduce_slice(1))
             self._phase_c()
             pending.append(self._all_reduce_slice(2))
+        elif self.masks:
+            if self.g_fwd is not None:
+                if frames is not self.static_frames:
+                    self.static_frames.copy_(frames, non_blocking=True)
+                if staged and dev.type == "cuda":
+                    self._release_staging(dev)
+                    staged = False
+                self.g_fwd.replay()
+                loss = self._mask_step_replayed(self.s_outs, self.s_grads, self.g_bwd, targets, num_boxes, False)
+            else:
+                loss = self._mask_loss(self.core(frames), targets, num_boxes, False)
+                self._mask_backward(loss)
         elif self.g_fwd is not None:
             if frames is not self.static_frames:
                 self.static_frames.copy_(frames, non_blocking=True)     # device or pinned-host source
