@@ -209,6 +209,28 @@ class MSDeformAttnEncFusedFunction(Function):
 _ENC_FUSED_CHOICE = {}
 _TILED_ENC_FUSED = _os.environ.get("TFB200_TILED_ENC_FUSED", "auto")     # "auto" | "1" | "0"
 
+# query tile of the encoder tile kernels (csrc/msda_enc_tma.cuh kEtTX x kEtTY)
+_ET_TILE_X, _ET_TILE_Y = 16, 8
+
+
+def enc_fused_domain(hw, n, s, m, d, len_q, backward=True) -> bool:
+    """Whether the fused-prologue tile kernels (``ms_deform_attn_{forward,backward}_enc_fused``) accept this geometry:
+    the host side of their geometry check (csrc/msda_kernels.cu ``et_prepare``), which the bindings turn into an error.
+    ``hw`` is the flat host list [H0, W0, ..., H3, W3]; four levels of four points, D = 32, queries == pixels, every level
+    at least 2 x 2 and at most 32767 on a side.  ``backward`` adds the backward kernel's limits: 12-bit window corners
+    (sides <= 4095) and 20-bit pixel indices (S < 2^20)."""
+    if len(hw) != 8 or d != 32 or len_q != s or n < 1 or m > 65535:
+        return False
+    if any(v < 2 or v > (4095 if backward else 32767) for v in hw):
+        return False
+    if backward and s >= 1 << 20:
+        return False
+    pairs = list(zip(hw[0::2], hw[1::2]))
+    if sum(h * w for h, w in pairs) != s:
+        return False
+    tiles = sum(-(-w // _ET_TILE_X) * -(-h // _ET_TILE_Y) for h, w in pairs)
+    return tiles * m * n <= 2 ** 31 - 1
+
 
 def encoder_fused_choice(key, time_fused, time_unfused) -> bool:
     """One-time decision per geometry between the fused-prologue tile kernels and the materialising path (sampling-prep

@@ -22,7 +22,7 @@ from torch import nn
 
 from .fused_linear import linear as fused_linear
 from .msda_function import (MSDeformAttnEncFunction, MSDeformAttnEncFusedFunction, MSDeformAttnFunction,
-                            MSDeformAttnFusedFunction, encoder_fused_choice)
+                            MSDeformAttnFusedFunction, enc_fused_domain, encoder_fused_choice)
 
 # fold sampling_prep into the MSDeformAttn kernels (csrc/msda_run.cuh PREP variants)
 _FUSED_PREP = os.environ.get("TFB200_FUSED_PREP", "0") != "0"
@@ -146,9 +146,11 @@ class MSDeformAttn(nn.Module):
             return fused_linear(out, self.output_proj.weight, self.output_proj.bias)
         if (hw is not None and len_q == len_in and proj.is_cuda and proj.dtype == torch.float32 and query_attn_mask is None
                 and not reference_points.requires_grad and reference_points.shape[-1] == 2 and levels == 4 and points == 4
-                and d_head == 32):
+                and d_head == 32 and enc_fused_domain([int(v) for pair in hw for v in pair], n, len_in, heads, d_head,
+                                                      len_q, backward=torch.is_grad_enabled())):
             # encoder call: the TMA tile kernels can evaluate softmax + locations in their tap pass; taken when that beats
-            # "sampling-prep kernel + op" on this geometry (timed once on the first eager call)
+            # "sampling-prep kernel + op" on this geometry (timed once on the first eager call).  Geometries outside the
+            # tile kernels' domain (a level under 2 x 2: an image side of 64 px or less) take the unfused route below.
             flat_hw = [int(v) for pair in hw for v in pair]
             key = (tuple(value.shape), tuple(flat_hw), value.device.index)
 
