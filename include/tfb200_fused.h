@@ -369,6 +369,23 @@ int tfb200_track_masks_f32(const float* logits, const int32_t* src, const int32_
                            int32_t* label, int T, int h, int w, int size_h, int size_w, int crop_h, int crop_w, int H,
                            int W, void* stream);
 
+/* Frame ingest (csrc/frame_ingest.cu; reference: the per-frame host work of datasets/tracking/mot17_sequence.py:68-81,
+ * i.e. Pillow's bilinear resize of the 8-bit image, to_tensor and Normalize): src [H][W][3] interleaved uint8 with
+ * src_row_stride bytes between rows (>= 3 * W)  ->  dst[c * dst_plane_stride + y * dst_row_stride + x] fp32, c < 3,
+ * y < h, x < w (strides in elements, so dst may be one image of a padded batch; 4-byte aligned).  Bit-identical to
+ * Pillow: per axis a device table of w (h) rows {lo, cnt, k_0 .. k_{ksize-1}} int32, weights quantised to 22 fractional
+ * bits; a pass is clamp((2^21 + sum_{j < cnt} pixel[lo + j] * k_j) >> 22, 0, 255), horizontal first, rounded to a byte
+ * between the passes.  xtab == NULL skips the horizontal pass and requires w == W, ytab == NULL likewise for rows; with
+ * both NULL the call only converts.  cnt_max_* is the largest cnt of that table (it bounds the shared-memory footprint
+ * of a tile); cnt_max > ksize is TFB200_E_SHAPE, as are non-positive sizes, and nothing is launched.  Every table row
+ * must satisfy lo >= 0, lo + cnt <= the input length and lo non-decreasing -- not checked, the host never reads the
+ * tables.  lut [3][256] fp32 maps the final byte of channel c to its normalised value.  Any ksize is handled until one
+ * output row's footprint exceeds 200 KB of shared memory (a reduction by several hundred: TFB200_E_SHAPE).        */
+int tfb200_frame_ingest_u8_f32(const uint8_t* src, int64_t src_row_stride, int H, int W, const int32_t* xtab,
+                               int ksize_x, int cnt_max_x, const int32_t* ytab, int ksize_y, int cnt_max_y,
+                               const float* lut, float* dst, int64_t dst_row_stride, int64_t dst_plane_stride, int h,
+                               int w, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1386,6 +1386,44 @@ at::Tensor track_masks(const at::Tensor& logits, const at::Tensor& src, const at
   return label;
 }
 
+// ---- frame ingest (csrc/frame_ingest.cu) ----
+// src [H, W, 3] uint8 (rows may be strided), xtab / ytab [w or h, 2 + ksize] int32 or None (that axis keeps its length),
+// lut [3, 256] fp32  ->  written into dst [3, h, w] fp32, a view whose last dimension is contiguous.  Allocates nothing.
+void frame_ingest(const at::Tensor& src, const c10::optional<at::Tensor>& xtab, int64_t cnt_max_x,
+                  const c10::optional<at::Tensor>& ytab, int64_t cnt_max_y, const at::Tensor& lut, at::Tensor dst) {
+  TORCH_CHECK(src.is_cuda() && src.scalar_type() == at::kByte, "frame_ingest src: uint8 CUDA tensor required (no CPU path)");
+  TORCH_CHECK(src.dim() == 3 && src.size(2) == 3 && src.size(0) > 0 && src.size(1) > 0 && src.stride(2) == 1 &&
+              src.stride(1) == 3 && src.stride(0) >= 3 * src.size(1),
+              "frame_ingest src: [H, W, 3] interleaved RGB rows required (only the row stride is free)");
+  check_f32(dst, "frame_ingest dst");
+  check_f32(lut, "frame_ingest lut");
+  TORCH_CHECK(dst.dim() == 3 && dst.size(0) == 3 && dst.size(1) > 0 && dst.size(2) > 0 && dst.stride(2) == 1,
+              "frame_ingest dst: [3, h, w] with a contiguous last dimension required");
+  TORCH_CHECK(lut.dim() == 2 && lut.size(0) == 3 && lut.size(1) == 256 && lut.is_contiguous(),
+              "frame_ingest lut: contiguous [3, 256] required");
+  TORCH_CHECK(dst.device() == src.device() && lut.device() == src.device(), "frame_ingest: tensors on different devices");
+  const int64_t H = src.size(0), W = src.size(1), h = dst.size(1), w = dst.size(2);
+  auto table = [&](const c10::optional<at::Tensor>& t, int64_t out_len, int64_t in_len, const char* what) -> const int32_t* {
+    if (!t.has_value() || !t->defined()) {
+      TORCH_CHECK(out_len == in_len, what, ": a table is required when the axis changes its length");
+      return nullptr;
+    }
+    TORCH_CHECK(t->is_cuda() && t->scalar_type() == at::kInt && t->device() == src.device() && t->is_contiguous() &&
+                t->dim() == 2 && t->size(0) == out_len && t->size(1) >= 3, what,
+                ": contiguous int32 CUDA table [output length, 2 + ksize] required");
+    return t->data_ptr<int32_t>();
+  };
+  const int32_t* xt = table(xtab, w, W, "frame_ingest xtab");
+  const int32_t* yt = table(ytab, h, H, "frame_ingest ytab");
+  const c10::cuda::CUDAGuard guard(src.device());
+  raise_rc(tfb200_frame_ingest_u8_f32(src.data_ptr<uint8_t>(), src.stride(0), int(H), int(W), xt,
+                                      xt ? int(xtab->size(1) - 2) : 0, int(cnt_max_x), yt,
+                                      yt ? int(ytab->size(1) - 2) : 0, int(cnt_max_y), lut.data_ptr<float>(),
+                                      dst.data_ptr<float>(), dst.stride(1), dst.stride(0), int(h), int(w),
+                                      c10::cuda::getCurrentCUDAStream().stream()),
+           "frame_ingest");
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "H100 (sm_90a) multi-scale deformable attention; drop-in for the reference extension";
   m.def("ms_deform_attn_forward", &ms_deform_attn_forward, "ms_deform_attn_forward");
@@ -1452,4 +1490,5 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mask_loss_forward", &mask_loss_forward);
   m.def("mask_loss_backward", &mask_loss_backward);
   m.def("track_masks", &track_masks);
+  m.def("frame_ingest", &frame_ingest);
 }

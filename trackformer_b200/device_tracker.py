@@ -160,7 +160,8 @@ class DeviceTracker(Tracker):
     # ---------------------------------------------------------------------------------------------------- step
     @torch.no_grad()
     def step(self, blob):
-        """One frame (tracker.py:266-548)."""
+        """One frame (tracker.py:266-548); `blob` as for `Tracker.step`: "img" or the raw uint8 "frame"."""
+        blob = self._with_image(blob)
         self._logger(f"FRAME: {self.frame_index + 1}")
         dev = self.device
         img = blob["img"].to(dev)

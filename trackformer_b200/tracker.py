@@ -151,8 +151,9 @@ class Tracker:
     """Drop-in for trackformer.models.tracker.Tracker (same arguments, tracker.py:19-20)."""
 
     def __init__(self, obj_detector, obj_detector_post, tracker_cfg, generate_attention_maps=False, logger=None,
-                 verbose=False):
+                 verbose=False, frame_ingest=None):
         self.obj_detector = obj_detector
+        self.frame_ingest = frame_ingest      # FrameIngest for blobs that carry a raw "frame"; made on first use if None
         self.obj_detector_post = obj_detector_post
         self.detection_obj_score_thresh = tracker_cfg["detection_obj_score_thresh"]
         self.track_obj_score_thresh = tracker_cfg["track_obj_score_thresh"]
@@ -218,6 +219,23 @@ class Tracker:
         if self._label is None or slot not in self._active:
             return None
         return self._label == int(self._state.ids[slot])
+
+    def _with_image(self, blob):
+        """The blob `step` works on.  A blob with "img" is returned as it is.  One with "frame" -- the raw uint8
+        [H, W, 3] RGB video frame, host or device -- gets "img", "size" and "orig_size" from the frame ingest
+        (frame_ingest.py: the reference's validation transform on the GPU, bit for bit); its other entries, e.g. the
+        public detections "dets" in original-image pixels, keep their meaning."""
+        if "frame" not in blob:
+            return blob
+        if "img" in blob:
+            raise ValueError('Tracker.step: the blob has both "img" and "frame"; give the pre-processed image or the '
+                             'raw uint8 frame, not both')
+        if self.frame_ingest is None:
+            from .frame_ingest import FrameIngest
+            self.frame_ingest = FrameIngest(self.device)
+        out = {k: v for k, v in blob.items() if k != "frame"}
+        out.update(self.frame_ingest(blob["frame"]))
+        return out
 
     def _detect(self, img, target, prev_features):
         """The detector call; with masks on, a segmentation model runs without its mask head (`detect`)."""
@@ -390,7 +408,9 @@ class Tracker:
     # ------------------------------------------------------------------------------------------------------ step
     @torch.no_grad()
     def step(self, blob):
-        """One frame (tracker.py:266-548)."""
+        """One frame (tracker.py:266-548).  `blob` holds the pre-processed "img" (with "orig_size", and "size" when
+        masks are on) or the raw uint8 "frame" (`_with_image`)."""
+        blob = self._with_image(blob)
         st = self._state
         released = []                            # slots freed during this step; recycled only afterwards
         hs_writes = {}                           # slot -> query index whose embedding the slot takes this frame
