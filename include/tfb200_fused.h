@@ -121,11 +121,23 @@ int tfb200_frozen_bn_act_bwd_f32(const float* dy, const float* y, const float* s
 int tfb200_tf32_linear_supported(int64_t M, int N, int K);
 int tfb200_tf32_linear_f32(const float* x, const float* w, const float* bias, float* y, int64_t M, int N, int K,
                            int relu, void* stream);
+/* The FFN's first Linear with its activation fused into the epilogue (models/deformable_transformer.py:282):
+ *   h = (a > 0 && keep(seed, row * N + col)) ? a / keep_prob : 0,   a = x . w^T + bias
+ * -- the mask of tfb200_relu_dropout_fwd_f32 on the same a, bit for bit.  seed_dev: the device int64 seed (read by
+ * the kernel, so a captured graph draws a fresh mask per replay); training == 0 is plain ReLU and needs no seed. */
+int tfb200_tf32_linear_relu_dropout_f32(const float* x, const float* w, const float* bias, const int64_t* seed_dev,
+                                        float* h, int64_t M, int N, int K, float keep_prob, int training, void* stream);
 /* The layer's two backward products on the same pipeline:
- *   dx[M][K]  = dy[M][N] . w[N][K]            (N % 32 == 0, K % 128 == 0)
+ *   dx[M][K]  = dy[M][N] . w[N][K]            (N % 32 == 0, K % 128 == 0; run as the forward product on wt = w^T,
+ *                                              which is written into the caller's [K][N] workspace wt first)
  *   dw[N][K]  = dy[M][N]^T . x[M][K]          (N, K % 128 == 0; the token axis M is split over all SMs, the partial
- *                                              products are added into dw by TMA reductions; dw is zero-filled here) */
-int tfb200_tf32_linear_dgrad_f32(const float* dy, const float* w, float* dx, int64_t M, int N, int K, void* stream);
+ *                                              products are added into dw by TMA reductions; dw is zero-filled here)
+ * dgrad_relu_dropout fuses the gradient of tfb200_tf32_linear_relu_dropout_f32's activation into the dgrad epilogue:
+ *   ga[M][K]  = h[M][K] > 0 ? (dy . w) / keep_prob : 0          (training == 0: keep_prob is taken as 1)      */
+int tfb200_tf32_linear_dgrad_f32(const float* dy, const float* w, float* wt, float* dx, int64_t M, int N, int K,
+                                 void* stream);
+int tfb200_tf32_linear_dgrad_relu_dropout_f32(const float* dy, const float* w, float* wt, const float* h, float* ga,
+                                              int64_t M, int N, int K, float keep_prob, int training, void* stream);
 int tfb200_tf32_linear_wgrad_f32(const float* dy, const float* x, float* dw, int64_t M, int N, int K, void* stream);
 
 /* out[r][c] = sigmoid(delta[r][c] + inverse_sigmoid(ref[r][c]))  for c < ref_dim (2 or 4), sigmoid(delta[r][c]) beyond;

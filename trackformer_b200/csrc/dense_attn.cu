@@ -23,25 +23,19 @@
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
+#include "dropout_hash.cuh"
 #include "launch_counter.h"
 
 namespace {
+
+using tfb200::keep_elem;        // keyed by the logical element index ((b * H + h) * Lq + q) * Lk + k
+using tfb200::keep_threshold;
 
 constexpr int kD = 32;              // channels per head
 constexpr int kWarps = 4;           // 16 rows (queries or keys) per warp
 constexpr int kRows = 16 * kWarps;  // rows per CTA
 constexpr int kTile = 64;           // keys (queries) per staged tile
 constexpr int kPitch = kD + 4;      // 144-byte rows: 16-byte aligned for cp.async, conflict-free fragment reads
-
-// the dropout hash of small_attn.cu / fused_norm.cu, keyed by the logical element index ((b * H + h) * Lq + q) * Lk + k
-__device__ __forceinline__ uint32_t mix32(uint32_t x) {
-  x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16;
-  return x;
-}
-__device__ __forceinline__ bool keep_elem(uint64_t seed, uint64_t idx, uint32_t keep_thresh) {
-  const uint32_t h = mix32(uint32_t(idx) ^ mix32(uint32_t(idx >> 32) + uint32_t(seed)) ^ uint32_t(seed >> 32) * 0x9e3779b9u);
-  return h < keep_thresh;
-}
 
 __device__ __forceinline__ uint32_t to_tf32(float x) {
   uint32_t r;
@@ -416,11 +410,6 @@ dense_attn_bwd_dkv_kernel(const float* __restrict__ q, const float* __restrict__
       *reinterpret_cast<float2*>(pv + 8 * j + 2 * t) = make_float2(av[j][2 * hr], av[j][2 * hr + 1]);
     }
   }
-}
-
-uint32_t keep_threshold(float keep_prob) {
-  const double t = double(keep_prob) * 4294967296.0;
-  return t >= 4294967295.0 ? 0xFFFFFFFFu : uint32_t(t);
 }
 
 bool aligned_view(const void* p, const int64_t* strides, int n) {

@@ -20,7 +20,11 @@
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
+#include "dropout_hash.cuh"
 #include "launch_counter.h"
+
+using tfb200::keep_elem;
+using tfb200::keep_threshold;
 
 namespace {
 
@@ -31,16 +35,6 @@ __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
-}
-
-// Counter-based keep decision for mask-free inverted dropout: a hash of (seed, element index) against a threshold.
-__device__ __forceinline__ uint32_t mix32(uint32_t x) {
-  x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16;
-  return x;
-}
-__device__ __forceinline__ bool keep_elem(uint64_t seed, uint64_t idx, uint32_t keep_thresh) {
-  const uint32_t h = mix32(uint32_t(idx) ^ mix32(uint32_t(idx >> 32) + uint32_t(seed)) ^ uint32_t(seed >> 32) * 0x9e3779b9u);
-  return h < keep_thresh;
 }
 
 // PACKS = ceil(C / 128): a lane owns float4 packs lane, lane + 32, ...; packs beyond C/4 are masked, so any C % 4 == 0
@@ -354,11 +348,6 @@ int grid_for(int64_t rows) {
 extern "C" {
 
 int tfb200_ln_partial_ctas(int64_t rows) { return grid_for(rows); }
-
-static uint32_t keep_threshold(float keep_prob) {
-  const double t = double(keep_prob) * 4294967296.0;
-  return t >= 4294967295.0 ? 0xffffffffu : uint32_t(t);
-}
 
 static int ln_forward(const float* x, const float* branch, const uint8_t* keep_mask, const int64_t* seed_dev,
                       const float* gamma, const float* beta, float* s_out, float* y, float* mean, float* rstd,

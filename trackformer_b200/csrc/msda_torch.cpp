@@ -375,6 +375,35 @@ at::Tensor tf32_linear(const at::Tensor& x, const at::Tensor& w, const c10::opti
   return y;
 }
 
+// h = dropout(relu(x . w^T + bias)) with the activation in the GEMM epilogue: relu_dropout_forward's mask on the same
+// pre-activation (flat index of the [M, N] output), one kernel instead of a GEMM and an elementwise pass
+at::Tensor tf32_linear_relu_dropout(const at::Tensor& x, const at::Tensor& w, const at::Tensor& bias,
+                                    const c10::optional<at::Tensor>& seed, double keep_prob, bool training) {
+  TORCH_CHECK(x.is_cuda() && w.is_cuda() && bias.is_cuda() && x.scalar_type() == at::kFloat &&
+                  w.scalar_type() == at::kFloat && bias.scalar_type() == at::kFloat && w.dim() == 2,
+              "tf32_linear_relu_dropout: fp32 CUDA tensors required");
+  const int64_t K = w.size(1), N = w.size(0);
+  TORCH_CHECK(x.dim() >= 1 && x.size(-1) == K && bias.numel() == N, "tf32_linear_relu_dropout: x[..., K], w[N, K], bias[N]");
+  const at::Tensor xc = x.contiguous(), wc = w.contiguous(), bc = bias.contiguous();
+  const int64_t M = xc.numel() / K;
+  const int64_t* sp = nullptr;
+  if (training) {
+    TORCH_CHECK(seed.has_value() && seed->is_cuda() && seed->scalar_type() == at::kLong && seed->numel() >= 1,
+                "tf32_linear_relu_dropout: training mode needs an int64 CUDA seed tensor");
+    sp = seed->data_ptr<int64_t>();
+  }
+  const c10::cuda::CUDAGuard guard(x.device());
+  auto sizes = xc.sizes().vec();
+  sizes.back() = N;
+  at::Tensor h = at::empty(sizes, xc.options());
+  if (M == 0) return h;
+  const int rc = tfb200_tf32_linear_relu_dropout_f32(xc.data_ptr<float>(), wc.data_ptr<float>(), bc.data_ptr<float>(), sp,
+                                                     h.data_ptr<float>(), M, int(N), int(K), float(keep_prob),
+                                                     training ? 1 : 0, c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "tf32_linear_relu_dropout failed (code ", rc, ")");
+  return h;
+}
+
 // dx = dy . w  and  dw = dy^T . x  of the same layer (csrc/tf32_gemm.cu, modes dgrad / wgrad)
 at::Tensor tf32_linear_dgrad(const at::Tensor& dy, const at::Tensor& w) {
   TORCH_CHECK(dy.is_cuda() && w.is_cuda() && dy.scalar_type() == at::kFloat && w.scalar_type() == at::kFloat && w.dim() == 2 &&
@@ -386,10 +415,35 @@ at::Tensor tf32_linear_dgrad(const at::Tensor& dy, const at::Tensor& w) {
   sizes.back() = K;
   at::Tensor dx = at::empty(sizes, g.options());
   if (M == 0) return dx;
-  const int rc = tfb200_tf32_linear_dgrad_f32(g.data_ptr<float>(), wc.data_ptr<float>(), dx.data_ptr<float>(), M, int(N),
-                                              int(K), c10::cuda::getCurrentCUDAStream().stream());
+  at::Tensor wt = at::empty({K, N}, wc.options());
+  const int rc = tfb200_tf32_linear_dgrad_f32(g.data_ptr<float>(), wc.data_ptr<float>(), wt.data_ptr<float>(),
+                                              dx.data_ptr<float>(), M, int(N), int(K),
+                                              c10::cuda::getCurrentCUDAStream().stream());
   TORCH_CHECK(rc == 0, "tf32_linear_dgrad failed (code ", rc, ")");
   return dx;
+}
+
+// ga = h > 0 ? (dy . w) / keep : 0 -- the dgrad of the FFN's second Linear with relu_dropout_backward in its epilogue;
+// h is tf32_linear_relu_dropout's output [..., K]
+at::Tensor tf32_linear_dgrad_relu_dropout(const at::Tensor& dy, const at::Tensor& w, const at::Tensor& h, double keep_prob,
+                                          bool training) {
+  TORCH_CHECK(dy.is_cuda() && w.is_cuda() && h.is_cuda() && dy.scalar_type() == at::kFloat &&
+                  w.scalar_type() == at::kFloat && h.scalar_type() == at::kFloat && w.dim() == 2 &&
+                  dy.size(-1) == w.size(0),
+              "tf32_linear_dgrad_relu_dropout: dy[..., N] against w[N, K]");
+  const at::Tensor g = dy.contiguous(), wc = w.contiguous(), hc = h.contiguous();
+  const int64_t N = wc.size(0), K = wc.size(1), M = g.numel() / N;
+  TORCH_CHECK(hc.numel() == M * K, "tf32_linear_dgrad_relu_dropout: h must hold M x K elements");
+  const c10::cuda::CUDAGuard guard(dy.device());
+  at::Tensor ga = at::empty_like(hc);
+  if (M == 0) return ga;
+  at::Tensor wt = at::empty({K, N}, wc.options());
+  const int rc = tfb200_tf32_linear_dgrad_relu_dropout_f32(g.data_ptr<float>(), wc.data_ptr<float>(), wt.data_ptr<float>(),
+                                                           hc.data_ptr<float>(), ga.data_ptr<float>(), M, int(N), int(K),
+                                                           float(keep_prob), training ? 1 : 0,
+                                                           c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "tf32_linear_dgrad_relu_dropout failed (code ", rc, ")");
+  return ga;
 }
 
 at::Tensor tf32_linear_wgrad(const at::Tensor& dy, const at::Tensor& x) {
@@ -1466,6 +1520,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("tf32_linear", &tf32_linear);
   m.def("tf32_linear_supported", &tf32_linear_supported);
   m.def("tf32_linear_dgrad", &tf32_linear_dgrad);
+  m.def("tf32_linear_relu_dropout", &tf32_linear_relu_dropout);
+  m.def("tf32_linear_dgrad_relu_dropout", &tf32_linear_dgrad_relu_dropout);
   m.def("tf32_linear_wgrad", &tf32_linear_wgrad);
   m.def("relu_dropout_forward", &relu_dropout_forward);
   m.def("relu_dropout_backward", &relu_dropout_backward);

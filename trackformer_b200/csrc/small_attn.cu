@@ -15,23 +15,18 @@
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
+#include "dropout_hash.cuh"
 #include "launch_counter.h"
 
 namespace {
+
+using tfb200::keep_elem;
+using tfb200::keep_threshold;
 
 constexpr int kD = 32;          // channels per head
 constexpr int kWarps = 8;       // queries (keys) per CTA
 constexpr int kTile = 32;       // keys (queries) per shared-memory tile
 constexpr int kPitch = kD + 1;  // odd pitch: lane = row reads are conflict-free
-
-__device__ __forceinline__ uint32_t mix32(uint32_t x) {
-  x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16;
-  return x;
-}
-__device__ __forceinline__ bool keep_elem(uint64_t seed, uint64_t idx, uint32_t keep_thresh) {
-  const uint32_t h = mix32(uint32_t(idx) ^ mix32(uint32_t(idx >> 32) + uint32_t(seed)) ^ uint32_t(seed >> 32) * 0x9e3779b9u);
-  return h < keep_thresh;
-}
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
@@ -243,11 +238,6 @@ small_attn_bwd_dkv_kernel(const float* __restrict__ q, const float* __restrict__
     dk[int64_t(ki) * dk_l + int64_t(b) * dk_b + h * kD + lane] = ak * scale;
     dv[int64_t(ki) * dv_l + int64_t(b) * dv_b + h * kD + lane] = av;
   }
-}
-
-uint32_t keep_threshold(float keep_prob) {
-  const double t = double(keep_prob) * 4294967296.0;
-  return t >= 4294967295.0 ? 0xFFFFFFFFu : uint32_t(t);
 }
 
 }  // namespace

@@ -23,7 +23,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import seeds, small_attention
-from .fused_linear import linear as fused_linear, relu_dropout
+from .fused_linear import ffn, ffn_fusable, linear as fused_linear, relu_dropout
 from .fused_norm import add_dropout_layernorm
 from .msda_module import MSDeformAttn
 from .util import refine_boxes
@@ -65,9 +65,12 @@ class DeformableTransformerEncoderLayer(nn.Module):
     with_pos_embed = staticmethod(_add_pos)
 
     def forward_ffn(self, src):
-        a = fused_linear(src, self.linear1.weight, self.linear1.bias)
-        h = relu_dropout(a, self.dropout2) if self.activation is F.relu else self.dropout2(self.activation(a))
-        ff = fused_linear(h, self.linear2.weight, self.linear2.bias)
+        if self.activation is F.relu and ffn_fusable(src, self.linear1, self.linear2, self.dropout2):
+            ff = ffn(src, self.linear1, self.linear2, self.dropout2)
+        else:
+            a = fused_linear(src, self.linear1.weight, self.linear1.bias)
+            h = relu_dropout(a, self.dropout2) if self.activation is F.relu else self.dropout2(self.activation(a))
+            ff = fused_linear(h, self.linear2.weight, self.linear2.bias)
         return add_dropout_layernorm(src, ff, self.dropout3, self.norm2)
 
     def forward(self, src, pos, reference_points, spatial_shapes, padding_mask=None):
