@@ -13,6 +13,7 @@
 #ifndef TFB200_FUSED_H_
 #define TFB200_FUSED_H_
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -380,6 +381,20 @@ int tfb200_mask_loss_bwd_f32(const float* logits, const int64_t* src, const uint
 int tfb200_track_masks_f32(const float* logits, const int32_t* src, const int32_t* ids, const int32_t* prev_label,
                            int32_t* label, int T, int h, int w, int size_h, int size_w, int crop_h, int crop_w, int H,
                            int W, void* stream);
+
+/* COCO run-length encodings of the masks label == ids[t] of a label map (csrc/mask_rle.cu; what pycocotools
+ * mask.encode(np.asfortranarray(label == ids[t]))["counts"] holds, for MOTS20Sequence.write_results,
+ * datasets/tracking/mots20_sequence.py:72-91).  label [H][W] int32 row-major (e.g. tfb200_track_masks_f32's output);
+ * ids [T] int32, >= 0, in any order, duplicates allowed (they get equal strings); label values that are not in ids,
+ * negative ones included, are background for every track.  Writes header [2 + 2T] int64 = {status, total bytes,
+ * offset[T], length[T]} and the T strings back to back into chars (offset[t] .. offset[t] + length[t]).  status bit 1:
+ * a negative id (its string is that of an empty mask); bit 2: total > chars_capacity, and chars is left untouched.
+ * tfb200_mask_rle_max_bytes(H, W, T) bounds the total for any label map.  workspace: tfb200_mask_rle_workspace_bytes
+ * bytes, 256-byte aligned (0 for a bad shape).  H * W <= 2^28, T <= 2^24.  T == 0 writes nothing.  Deterministic.  */
+size_t tfb200_mask_rle_workspace_bytes(int H, int W, int T);
+int64_t tfb200_mask_rle_max_bytes(int H, int W, int T);
+int tfb200_mask_rle_i32(const int32_t* label, const int32_t* ids, int H, int W, int T, void* workspace,
+                        size_t workspace_bytes, int64_t* header, char* chars, int64_t chars_capacity, void* stream);
 
 /* Frame ingest (csrc/frame_ingest.cu; reference: the per-frame host work of datasets/tracking/mot17_sequence.py:68-81,
  * i.e. Pillow's bilinear resize of the 8-bit image, to_tensor and Normalize): src [H][W][3] interleaved uint8 with

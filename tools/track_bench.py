@@ -11,7 +11,10 @@ exactly `--tracks` tracks, afterwards every track is kept and no new ones start.
 DeviceTracker over the CUDA-graph detector, each running the mask head on the rows the frame's decisions keep and
 resolving the masks into one label map, against the reference-shaped work for the same frame -- the full forward with
 `pred_masks` for every query row plus PostProcessSegm(return_probs=True), which upsamples every row to the image and
-copies it to the host.
+copies it to the host.  Each tracker runs twice, frame by frame in turn: with the results' bool masks (the label map
+read back) and with `mask_rle=True` (COCO RLE strings made on the device); per arm the line gives the latency, the
+device-to-host bytes of the masks per frame as counted from what arrived, and the host bytes the results' masks hold
+at the end (bool arrays' nbytes against the strings' lengths).
 
 Prints one JSON line; tools/README.md lists it among the measurement aids.  Not a bench.py arm.
 """
@@ -71,15 +74,15 @@ def main():
             b["size"] = size
         return b
 
-    def run(detector, tracker_cls=Tracker):
+    def start(detector, tracker_cls=Tracker, **kwargs):
+        """a tracker whose first frame starts exactly --tracks tracks"""
         post = DeformablePostProcess()
         posts = {"bbox": post}
         if args.masks:
             from trackformer_b200.segmentation import PostProcessSegm
             posts["segm"] = PostProcessSegm()
-        tr = tracker_cls(detector, posts, cfg, False)
+        tr = tracker_cls(detector, posts, cfg, False, **kwargs)
         tr.reset()
-        # frame 0: start exactly --tracks tracks
         with torch.no_grad():
             out = detector(frames[0].to(dev), None, None)[0]
         rows = post.packed(out, size.to(dev))[0].cpu().numpy()
@@ -89,22 +92,27 @@ def main():
         tr.step(blob(0))
         tr.detection_obj_score_thresh = 2.0
         assert len(tr.tracks) == args.tracks, len(tr.tracks)
+        return tr
+
+    def timed_step(tr, i):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        tr.step(blob(i + 1))
+        torch.cuda.synchronize()
+        return (time.perf_counter() - t0) * 1e3
+
+    def run(detector, tracker_cls=Tracker):
+        tr = start(detector, tracker_cls)
         times = []
         for i in range(args.warmup + args.frames):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            tr.step(blob(i + 1))
-            torch.cuda.synchronize()
+            t = timed_step(tr, i)
             if i >= args.warmup:
-                times.append((time.perf_counter() - t0) * 1e3)
+                times.append(t)
         assert len(tr.tracks) == args.tracks
-        if args.masks:
-            head_rows.append(int((tr._result_rows >= 0).sum()))
         return times
 
-    head_rows = []
     if args.masks:
-        print(json.dumps(masks_line(args, model, frames, size, dev, run, head_rows)))
+        print(json.dumps(masks_line(args, model, frames, size, dev, start, timed_step)))
         return
     det = GraphedDetector(model, bucket=args.bucket)
     graphed = run(det)
@@ -128,10 +136,11 @@ def main():
     print(json.dumps(line))
 
 
-def masks_line(args, model, frames, size, dev, run, head_rows):
+def masks_line(args, model, frames, size, dev, start, timed_step):
     from trackformer_b200.device_tracker import DeviceTracker
     from trackformer_b200.graphed_detector import GraphedDetector
     from trackformer_b200.segmentation import PostProcessSegm
+    from trackformer_b200.tracker import Tracker
 
     # the reference-shaped work of one frame: full forward (pred_masks for all rows) + PostProcessSegm to the host
     post = PostProcessSegm()
@@ -152,24 +161,53 @@ def masks_line(args, model, frames, size, dev, run, head_rows):
         n_rows = args.tracks + model.num_queries
         del out, o
     torch.cuda.empty_cache()
-    host = run(GraphedDetector(model, bucket=args.bucket))
-    device = run(GraphedDetector(model, bucket=args.bucket), DeviceTracker)
+
+    # four arms -- {Tracker, DeviceTracker} x {bool masks, RLE masks} -- each over its own CUDA-graph detector, stepped
+    # in turn frame by frame so that they share the machine's state
+    arms = {}
+    for name, cls, rle in (("graph_masks", Tracker, False), ("graph_masks_rle", Tracker, True),
+                           ("graph_device_tracker_masks", DeviceTracker, False),
+                           ("graph_device_tracker_masks_rle", DeviceTracker, True)):
+        arms[name] = {"tracker": start(GraphedDetector(model, bucket=args.bucket), cls, mask_rle=rle), "rle": rle,
+                      "times": [], "d2h": []}
+    label_bytes = args.height * args.width * 4
+    for i in range(args.warmup + args.frames):
+        for arm in arms.values():
+            tr = arm["tracker"]
+            t = timed_step(tr, i)
+            if i < args.warmup:
+                continue
+            arm["times"].append(t)
+            # device-to-host bytes of the frame's masks, counted from what arrived: the label map, or the RLE header
+            # (status, total, offset and length per result) plus the strings
+            frame = [r[tr.frame_index - 1] for r in tr.results.values() if tr.frame_index - 1 in r]
+            if arm["rle"]:
+                arm["d2h"].append(8 * (2 + 2 * len(frame)) + sum(len(e["mask"]["counts"]) for e in frame))
+            else:
+                arm["d2h"].append(label_bytes)
+    rows_d2h = {False: n_rows * 6 * 4, True: (8 + 8 * n_rows) * 4}        # the frame's result rows, per tracker kind
 
     def stats(t):
         return {"median": float(np.median(t)), "p10": float(np.percentile(t, 10)), "p90": float(np.percentile(t, 90))}
-    label_bytes = args.height * args.width * 4
-    return {
+    line = {
         "what": "Tracker.step latency with segmentation masks, host frame in -> results (with masks) out",
         "frames": args.frames, "warmup": args.warmup,
         "config": {"workload": f"segmentation tracking 1x3x{args.height}x{args.width}, {args.tracks} track + "
                                f"{model.num_queries} object queries", "bucket": args.bucket, "tf32": not args.no_tf32},
-        "graph_masks_ms": stats(host), "graph_device_tracker_masks_ms": stats(device),
         "reference_shaped_forward_plus_postprocess_segm_ms": stats(full),
-        "head_rows_per_frame": head_rows, "head_rows_per_frame_reference_shaped": n_rows,
-        "d2h_bytes_per_frame": int(n_rows * 6 * 4 + label_bytes),
-        "d2h_bytes_per_frame_device_tracker": int((8 + 8 * n_rows) * 4 + label_bytes),
+        "head_rows_reference_shaped": n_rows,
         "d2h_bytes_per_frame_reference_shaped": int(n_rows * args.height * args.width * 4),
     }
+    for name, arm in arms.items():
+        tr = arm["tracker"]
+        assert len(tr.tracks) == args.tracks
+        held = sum(len(e["mask"]["counts"]) if arm["rle"] else e["mask"].nbytes
+                   for r in tr.results.values() for e in r.values())
+        line[name] = {"ms": stats(arm["times"]), "head_rows_last_frame": int((tr._result_rows >= 0).sum()),
+                      "mask_d2h_bytes_per_frame": stats(arm["d2h"]),
+                      "d2h_bytes_per_frame": float(np.median(arm["d2h"])) + rows_d2h[isinstance(tr, DeviceTracker)],
+                      "results_mask_host_bytes": int(held), "results_frames": tr.frame_index}
+    return line
 
 
 if __name__ == "__main__":

@@ -1440,6 +1440,42 @@ at::Tensor track_masks(const at::Tensor& logits, const at::Tensor& src, const at
   return label;
 }
 
+// ---- COCO RLE strings of a label map's per-track masks (csrc/mask_rle.cu) ----
+// label [H, W] int32, ids [T] int32 on one device -> T bytes objects.  Two device-to-host copies: the header (offsets,
+// lengths) and then exactly the string bytes; the label map stays on the device.
+std::vector<pybind11::bytes> mask_rle(const at::Tensor& label, const at::Tensor& ids) {
+  TORCH_CHECK(label.is_cuda() && label.scalar_type() == at::kInt && label.dim() == 2,
+              "mask_rle label: int32 CUDA tensor [H, W] required");
+  TORCH_CHECK(ids.is_cuda() && ids.scalar_type() == at::kInt && ids.dim() == 1 && ids.device() == label.device(),
+              "mask_rle ids: int32 CUDA tensor [T] on the label map's device required");
+  const int64_t H = label.size(0), W = label.size(1), T = ids.size(0);
+  TORCH_CHECK(H > 0 && W > 0 && H * W <= (int64_t(1) << 28) && T <= (int64_t(1) << 24),
+              "mask_rle: H, W > 0, H * W <= 2^28 and T <= 2^24 required");
+  if (T == 0) return {};
+  const c10::cuda::CUDAGuard guard(label.device());
+  const at::Tensor lc = label.contiguous(), ic = ids.contiguous();
+  const auto u8 = lc.options().dtype(at::kByte);
+  const size_t ws_bytes = tfb200_mask_rle_workspace_bytes(int(H), int(W), int(T));
+  const int64_t cap = tfb200_mask_rle_max_bytes(int(H), int(W), int(T));
+  at::Tensor ws = at::empty({int64_t(ws_bytes)}, u8);
+  at::Tensor chars = at::empty({cap}, u8);
+  at::Tensor header = at::empty({2 + 2 * T}, lc.options().dtype(at::kLong));
+  raise_rc(tfb200_mask_rle_i32(lc.data_ptr<int32_t>(), ic.data_ptr<int32_t>(), int(H), int(W), int(T), ws.data_ptr(),
+                               ws_bytes, header.data_ptr<int64_t>(), reinterpret_cast<char*>(chars.data_ptr()), cap,
+                               c10::cuda::getCurrentCUDAStream().stream()),
+           "mask_rle");
+  const at::Tensor h = header.cpu();
+  const int64_t* hp = h.data_ptr<int64_t>();
+  TORCH_CHECK(!(hp[0] & 1), "mask_rle: ids must be >= 0");
+  TORCH_CHECK(hp[0] == 0, "mask_rle: ", hp[1], " string bytes exceed the bound of ", cap);
+  const at::Tensor s = chars.narrow(0, 0, hp[1]).cpu();
+  const char* sp = reinterpret_cast<const char*>(s.data_ptr());
+  std::vector<pybind11::bytes> out;
+  out.reserve(size_t(T));
+  for (int64_t t = 0; t < T; ++t) out.emplace_back(sp + hp[2 + t], size_t(hp[2 + T + t]));
+  return out;
+}
+
 // ---- frame ingest (csrc/frame_ingest.cu) ----
 // src [H, W, 3] uint8 (rows may be strided), xtab / ytab [w or h, 2 + ksize] int32 or None (that axis keeps its length),
 // lut [3, 256] fp32  ->  written into dst [3, h, w] fp32, a view whose last dimension is contiguous.  Allocates nothing.
@@ -1546,5 +1582,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mask_loss_forward", &mask_loss_forward);
   m.def("mask_loss_backward", &mask_loss_backward);
   m.def("track_masks", &track_masks);
+  m.def("mask_rle", &mask_rle);
   m.def("frame_ingest", &frame_ingest);
 }

@@ -26,7 +26,9 @@ where it takes a new embedding (`hs_writes`), so after the decisions the mask he
 (`mask_logits` of a segmentation model, or `GraphedDetector.mask_logits`), and `resolve_track_masks`
 (csrc/track_masks.cu on the GPU) resolves the overlaps of all active tracks at the original resolution into one label
 map -- the frame's only extra read-back.  A track that keeps its previous mask reads it from the previous label map,
-which stays on the device.  `results[id][frame]["mask"]` is the reference's bool array [H, W]; `Track.mask` is the
+which stays on the device.  `results[id][frame]["mask"]` is the reference's bool array [H, W], or with
+`mask_rle=True` its COCO RLE dict (`mots.encode`'s format, what the MOTS20 result file holds), made from the device label
+map by csrc/mask_rle.cu so that only the strings are read back (`mots.decode` gives the array); `Track.mask` is the
 frame's resolved bool mask for active tracks and None for inactive ones (the reference keeps an inactive track's last
 mask, which nothing reads: a track that comes back always takes a new one).
 """
@@ -38,6 +40,7 @@ import torch.nn.functional as F
 from scipy.optimize import linear_sum_assignment
 
 from .graphed_detector import GraphedDetector
+from .mots import label_map_rle
 from .segmentation import resolve_track_masks
 
 __all__ = ["Tracker", "Track", "nms_keep", "pairwise_iou"]
@@ -151,7 +154,7 @@ class Tracker:
     """Drop-in for trackformer.models.tracker.Tracker (same arguments, tracker.py:19-20)."""
 
     def __init__(self, obj_detector, obj_detector_post, tracker_cfg, generate_attention_maps=False, logger=None,
-                 verbose=False, frame_ingest=None):
+                 verbose=False, frame_ingest=None, mask_rle=False):
         self.obj_detector = obj_detector
         self.frame_ingest = frame_ingest      # FrameIngest for blobs that carry a raw "frame"; made on first use if None
         self.obj_detector_post = obj_detector_post
@@ -171,6 +174,7 @@ class Tracker:
             # the reference asserts the same for the deformable model (tracker.py:38)
             raise ValueError("Generation of attention maps not possible for deformable DETR.")
         self.masks = "segm" in obj_detector_post
+        self.mask_rle = bool(mask_rle)        # results' "mask": COCO RLE dicts (mots.label_map_rle) instead of bool arrays
         self.generate_attention_maps = False
         self._logger = logger if logger is not None else (lambda *log_strs: None)
         self._verbose = verbose
@@ -256,10 +260,11 @@ class Tracker:
 
     def _resolve_masks(self, det_out, src_rows, ids, blob, orig):
         """Masks of the active tracks (ids, in list order) of this frame: `src_rows[t]` is the query row whose mask
-        track t takes, -1 to keep its previous one.  Returns the host label map [H, W] (the one read-back) or None."""
+        track t takes, -1 to keep its previous one.  Returns the results' masks in `ids` order: bool arrays [H, W] from
+        the host label map (the one read-back), or with `mask_rle` the COCO RLEs made from the device label map."""
         if not len(ids):
             self._label = None
-            return None
+            return []
         stale = any(r < 0 for r in src_rows)
         if stale and (self._label is None or tuple(self._label.shape) != tuple(orig)):
             # the reference fails here too (torch.stack of masks of different sizes, tracker.py:510)
@@ -276,7 +281,10 @@ class Tracker:
         label = resolve_track_masks(logits, src, [int(i) for i in ids], self._label if stale else None, size, size,
                                     orig)
         self._label = label
-        return label.cpu().numpy()
+        if self.mask_rle:
+            return label_map_rle(label, ids)
+        host = label.cpu().numpy()
+        return [host == i for i in ids]
 
     def _take_slot(self):
         if not self._free:
@@ -530,14 +538,14 @@ class Tracker:
 
         # ---- masks (tracker.py:509-521) and results (tracker.py:533-548)
         self._result_rows = np.asarray([hs_writes.get(s, -1) for s in self._active], np.int64)
-        label = None
+        masks = None
         if self.masks:
-            label = self._resolve_masks(det_out, self._result_rows, st.ids[self._active], blob, (height, width))
-        for s in self._active:
+            masks = self._resolve_masks(det_out, self._result_rows, st.ids[self._active], blob, (height, width))
+        for k, s in enumerate(self._active):
             box = st.pos[s] if self.obj_detector.overflow_boxes else _clip(st.pos[s], height, width)
             entry = {"bbox": box.copy(), "score": np.array(st.score[s]), "obj_ind": int(st.obj_ind[s])}
-            if label is not None:
-                entry["mask"] = label == st.ids[s]
+            if masks is not None:
+                entry["mask"] = masks[k]
             self.results.setdefault(int(st.ids[s]), {})[self.frame_index] = entry
         for s in self._inactive:
             st.count_inactive[s] += 1
