@@ -255,6 +255,14 @@ int tfb200_dense_attn_bwd_f32(const float* q, const float* k, const float* v, co
                               const int64_t* seed_dev, const float* out, const float* lse, const float* dout,
                               float* dq, float* dk, float* dv, float* delta_ws, int B, int H, int Lq, int Lk,
                               const int64_t* strides16, float scale, float keep_prob, void* stream);
+/* The attention probabilities of the forward averaged over heads (nn.MultiheadAttention's need_weights=True,
+ * average_attn_weights=True): weights [B][Lq][Lk] (contiguous) = (1/H) sum_h exp(scale q_h . k_h - lse[b][h][q]),
+ * from the same q / k views (strides4 = {q_l, q_b, k_l, k_b}, alignment as above) and the lse [B][H][Lq] of
+ * tfb200_dense_attn_fwd_f32; dropout does not enter.  Ignored keys (key_pad nonzero) get exactly 0, and so does every
+ * key of a query whose keys are all ignored.  One launch, no atomics: bitwise reproducible.  B <= 65535.          */
+int tfb200_dense_attn_weights_f32(const float* q, const float* k, const uint8_t* key_pad, const float* lse,
+                                  float* weights, int B, int H, int Lq, int Lk, const int64_t* strides4, float scale,
+                                  void* stream);
 
 /* One frame of the online tracker's bookkeeping on the device (csrc/track_step.cu; reference models/tracker.py:266-548:
  * score thresholds 337-373 / 425-436, both NMS passes 388-406 / 494-515, public-detection gating 122-164, ReID 166-264,

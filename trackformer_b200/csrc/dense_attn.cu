@@ -412,6 +412,80 @@ dense_attn_bwd_dkv_kernel(const float* __restrict__ q, const float* __restrict__
   }
 }
 
+// ---------------------------------------------------------------------------------------------- head-averaged weights
+// W[b, r, c] = (1/H) sum_h exp(scale q_h[r] . k_h[c] - lse[b, h, r]): the probabilities of the forward, averaged over
+// heads (nn.MultiheadAttention's need_weights=True, average_attn_weights=True), from the forward's own log-sum-exp.
+// CTA = 64 rows x 64 keys of one image, 16 x 16 threads with 4 x 4 outputs each (rows ty + 16i, keys tx + 16j); the
+// head loop stages that head's q / k tiles in shared memory and accumulates in registers, so every output element is
+// written once, in a fixed order: no atomics, bitwise reproducible.  Scores are fp32 FMA dot products (32 channels).
+constexpr int kWTile = 64;
+constexpr int kWPitch = kD + 1;        // odd pitch: the 16 keys / 2 rows a warp reads per channel hit distinct banks
+
+__global__ void __launch_bounds__(256)
+dense_attn_weights_kernel(const float* __restrict__ q, const float* __restrict__ k, const uint8_t* __restrict__ key_pad,
+                          const float* __restrict__ lse, float* __restrict__ weights, int H, int Lq, int Lk, float scale,
+                          int64_t q_l, int64_t q_b, int64_t k_l, int64_t k_b) {
+  __shared__ float sq[kWTile][kWPitch];
+  __shared__ float sk[kWTile][kWPitch];
+  __shared__ float s_lse[kWTile];
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int c0 = blockIdx.x * kWTile, r0 = blockIdx.y * kWTile, b = blockIdx.z;
+  float acc[4][4] = {};
+  for (int h = 0; h < H; ++h) {
+    for (int i = threadIdx.x; i < kWTile * (kD / 4); i += 256) {
+      const int r = i >> 3, c = (i & 7) * 4;
+      float4 x = make_float4(0.f, 0.f, 0.f, 0.f), y = x;
+      if (r0 + r < Lq) x = __ldg(reinterpret_cast<const float4*>(q + int64_t(r0 + r) * q_l + int64_t(b) * q_b + h * kD + c));
+      if (c0 + r < Lk) y = __ldg(reinterpret_cast<const float4*>(k + int64_t(c0 + r) * k_l + int64_t(b) * k_b + h * kD + c));
+      sq[r][c] = x.x * scale; sq[r][c + 1] = x.y * scale; sq[r][c + 2] = x.z * scale; sq[r][c + 3] = x.w * scale;
+      sk[r][c] = y.x; sk[r][c + 1] = y.y; sk[r][c + 2] = y.z; sk[r][c + 3] = y.w;
+    }
+    if (threadIdx.x < kWTile) {
+      const int r = r0 + threadIdx.x;
+      s_lse[threadIdx.x] = r < Lq ? __ldg(lse + (int64_t(b) * H + h) * Lq + r) : INFINITY;
+    }
+    __syncthreads();
+    float s[4][4] = {};
+#pragma unroll 8
+    for (int c = 0; c < kD; ++c) {
+      float a[4], kk[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = sq[ty + 16 * i][c];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) kk[j] = sk[tx + 16 * j][c];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) s[i][j] = fmaf(a[i], kk[j], s[i][j]);
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float ls = s_lse[ty + 16 * i];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[i][j] += ls == INFINITY ? 0.f : expf(s[i][j] - ls);   // fully masked row -> 0
+    }
+    __syncthreads();                   // the tiles are restaged for the next head
+  }
+  const float inv_h = 1.f / float(H);
+  bool live[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int c = c0 + tx + 16 * j;
+    live[j] = c < Lk && !(key_pad && key_pad[int64_t(b) * Lk + c]);
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int r = r0 + ty + 16 * i;
+    if (r >= Lq) continue;
+    float* w = weights + (int64_t(b) * Lq + r) * Lk;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int c = c0 + tx + 16 * j;
+      if (c < Lk) w[c] = live[j] ? acc[i][j] * inv_h : 0.f;
+    }
+  }
+}
+
 bool aligned_view(const void* p, const int64_t* strides, int n) {
   if (reinterpret_cast<uintptr_t>(p) & 15u) return false;
   for (int i = 0; i < n; ++i)
@@ -434,6 +508,19 @@ extern "C" int tfb200_dense_attn_fwd_f32(const float* q, const float* k, const f
   const dim3 grid((Lq + kRows - 1) / kRows, B * H);
   dense_attn_fwd_kernel<<<grid, kWarps * 32, 0, cudaStream_t(stream)>>>(q, k, v, key_pad, seed_dev, out, lse, H, Lq, Lk,
                                                                        scale, 1.f / keep_prob, keep_threshold(keep_prob), st);
+  msda_b200_count_launches(1);
+  return int(cudaGetLastError());
+}
+
+extern "C" int tfb200_dense_attn_weights_f32(const float* q, const float* k, const uint8_t* key_pad, const float* lse,
+                                             float* weights, int B, int H, int Lq, int Lk, const int64_t* strides4,
+                                             float scale, void* stream) {
+  if (!q || !k || !lse || !weights || !strides4) return TFB200_E_NULLPTR;
+  if (B < 1 || H < 1 || Lq < 1 || Lk < 1 || B > 65535 || (Lq + kWTile - 1) / kWTile > 65535) return TFB200_E_SHAPE;
+  if (!aligned_view(q, strides4, 2) || !aligned_view(k, strides4 + 2, 2)) return TFB200_E_SHAPE;
+  const dim3 grid((Lk + kWTile - 1) / kWTile, (Lq + kWTile - 1) / kWTile, B);
+  dense_attn_weights_kernel<<<grid, 256, 0, cudaStream_t(stream)>>>(q, k, key_pad, lse, weights, H, Lq, Lk, scale,
+                                                                     strides4[0], strides4[1], strides4[2], strides4[3]);
   msda_b200_count_launches(1);
   return int(cudaGetLastError());
 }

@@ -591,6 +591,25 @@ std::vector<at::Tensor> dense_attention_backward(const at::Tensor& q, const at::
   return {dq, dk, dv};
 }
 
+// Head-averaged attention probabilities [B, Lq, Lk] of a dense_attention_forward call, from its q / k views and lse.
+at::Tensor dense_attention_weights(const at::Tensor& q, const at::Tensor& k, const c10::optional<at::Tensor>& key_pad,
+                                   const at::Tensor& lse, double scale) {
+  check_dense_shapes(q, k, k);
+  const int64_t Lq = q.size(0), B = q.size(1), H = q.size(2), Lk = k.size(0);
+  TORCH_CHECK(lse.is_cuda() && lse.scalar_type() == at::kFloat && lse.is_contiguous() && lse.numel() == B * H * Lq,
+              "dense_attention_weights: lse must be the forward's [B, H, Lq]");
+  const c10::cuda::CUDAGuard guard(q.device());
+  at::Tensor weights = at::empty({B, Lq, Lk}, q.options());
+  at::Tensor kpc;
+  const uint8_t* kp = dense_key_pad(key_pad, kpc, B, Lk, q);
+  const int64_t st[4] = {q.stride(0), q.stride(1), k.stride(0), k.stride(1)};
+  const int rc = tfb200_dense_attn_weights_f32(q.data_ptr<float>(), k.data_ptr<float>(), kp, lse.data_ptr<float>(),
+                                               weights.data_ptr<float>(), int(B), int(H), int(Lq), int(Lk), st,
+                                               float(scale), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "dense_attention_weights failed (code ", rc, ")");
+  return weights;
+}
+
 // boxes = sigmoid(delta + inverse_sigmoid(ref)) (csrc/box_refine.cu); delta [..., 4], ref [..., 2 or 4]
 at::Tensor refine_boxes_forward(const at::Tensor& delta, const at::Tensor& ref, double eps) {
   TORCH_CHECK(delta.is_cuda() && ref.is_cuda() && delta.scalar_type() == at::kFloat && ref.scalar_type() == at::kFloat &&
@@ -1551,6 +1570,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("small_attention_backward", &small_attention_backward);
   m.def("dense_attention_forward", &dense_attention_forward);
   m.def("dense_attention_backward", &dense_attention_backward);
+  m.def("dense_attention_weights", &dense_attention_weights);
   m.def("refine_boxes_forward", &refine_boxes_forward);
   m.def("refine_boxes_backward", &refine_boxes_backward);
   m.def("tf32_linear", &tf32_linear);

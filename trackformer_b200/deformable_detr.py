@@ -59,6 +59,9 @@ class DETR(nn.Module):
         self.input_proj = nn.Conv2d(backbone.num_channels[-1], self.hidden_dim, kernel_size=1)
         self.backbone = backbone
         self.aux_loss = aux_loss
+        # the last decoder layer's head-averaged cross-attention weights as out["attention_maps"] [B, Q, h, w] (the
+        # reference tracker's generate_attention_maps); a vanilla-transformer switch, set by Tracker
+        self.generate_attention_maps = False
 
     @property
     def hidden_dim(self):
@@ -77,7 +80,9 @@ class DETR(nn.Module):
         decoder input is ``track_query_hs_embeds``.  ``prev_features`` is accepted (the tracker passes it) and ignored:
         vanilla DETR has no multi-frame path.  ``track_query_padding`` [K] per image marks filler track queries, hidden
         from the others as self-attention keys (GraphedDetector, TrainStep).  Unlike the reference, the targets'
-        ``track_query_hs_embeds`` are not overwritten with the full decoder input rows."""
+        ``track_query_hs_embeds`` are not overwritten with the full decoder input rows.  With
+        ``generate_attention_maps`` set, ``out["attention_maps"]`` holds the last decoder layer's cross-attention
+        weights averaged over heads, [B, Q, h, w] on the grid of the transformer memory."""
         if not isinstance(samples, NestedTensor):
             samples = nested_tensor_from_tensor_list(samples)
         features, pos = self.backbone(samples)
@@ -94,11 +99,14 @@ class DETR(nn.Module):
             if "track_query_padding" in targets[0]:
                 filler = torch.stack([t["track_query_padding"] for t in targets])
                 tgt_pad = torch.cat([filler, filler.new_zeros(bs, self.num_queries)], 1)
-        hs, hs_without_norm, memory = self.transformer(src, mask, query_embed, pos[-1], tgt,
-                                                       tgt_key_padding_mask=tgt_pad)
+        res = self.transformer(src, mask, query_embed, pos[-1], tgt, tgt_key_padding_mask=tgt_pad,
+                               need_weights=self.generate_attention_maps)
+        hs, hs_without_norm, memory = res[:3]
         outputs_class = self.class_embed(hs)
         outputs_coord = self.bbox_embed(hs).sigmoid()
         out = {"pred_logits": outputs_class[-1], "pred_boxes": outputs_coord[-1], "hs_embed": hs_without_norm[-1]}
+        if self.generate_attention_maps:
+            out["attention_maps"] = res[3]
         if self.aux_loss:
             out["aux_outputs"] = self._set_aux_loss(outputs_class, outputs_coord)
         return out, targets, features, memory, hs

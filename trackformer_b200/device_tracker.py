@@ -17,7 +17,8 @@ CUDA only: on CPU tensors `step` raises (use `Tracker`, whose bookkeeping is hos
 Segmentation masks work as in `Tracker`: word 7 of each result row is the query row whose embedding -- and so whose
 mask -- the track took this frame (-1: it keeps its previous mask), so the mask head runs on those rows after the
 read-back and the same resolution kernel writes the frame's label map (and, with `mask_rle=True`, csrc/mask_rle.cu the
-results' COCO RLEs from it).
+results' COCO RLEs from it).  Attention maps (`generate_attention_maps=True`) take the same rows: after the read-back
+the maps of those rows are gathered on the device and read back in one copy; with the switch off nothing is added.
 
 Differences a user can see: the debug logger receives the FRAME and INIT TRACK IDS lines only (the per-decision lines
 of tracker.py:375-379, 399-402, 232-235 would need the decisions on the host); `tracks` / `inactive_tracks` between
@@ -80,6 +81,7 @@ class DeviceTracker(Tracker):
         """tracker.py:71-80"""
         self._bufs = None
         self._label = None
+        self._maps = {}
         self._cur = 0                                 # index of the state buffer holding the current state
         self._n_active = self._n_inactive = self._n_query = 0
         self._host_view = None
@@ -230,13 +232,17 @@ class DeviceTracker(Tracker):
         body = out[8:8 + 8 * n_results].reshape(n_results, 8)
         fbody = body.view(np.float32)
         self._result_rows = body[:, 7].astype(np.int64)
-        masks = None
+        masks = maps = None
         if self.masks:
             masks = self._resolve_masks(det_out, self._result_rows, body[:, 0], blob, (height, width))
+        if self.generate_attention_maps:
+            maps = self._attention_maps(det_out, self._result_rows, body[:, 0])
         for k in range(n_results):
             entry = {"bbox": fbody[k, 3:7].copy(), "score": np.array(fbody[k, 2]), "obj_ind": int(body[k, 1])}
             if masks is not None:
                 entry["mask"] = masks[k]
+            if maps is not None and maps[k] is not None:
+                entry["attention_map"] = maps[k].copy()
             self.results.setdefault(int(body[k, 0]), {})[self.frame_index] = entry
         if track_num > self.track_num:
             self._logger(f"INIT TRACK IDS (detection_obj_score_thresh={self.detection_obj_score_thresh}): "

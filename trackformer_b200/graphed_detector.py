@@ -18,6 +18,9 @@ For segmentation models (those with `detect` / `mask_logits`, segmentation.py) t
 without the mask head, so `pred_masks` is not returned either; `mask_logits(rows)` runs the head eagerly on the rows
 the tracker asks for, from the static buffers of the last call.
 `use_graphs=False` keeps the padding but runs the model eagerly (used by the CPU tests of the padding logic).
+
+With the vanilla model's `generate_attention_maps` switch on, the switch is part of the plan key: the captured graph
+computes the maps as one more static output, and `out["attention_maps"]` drops the filler rows like the other outputs.
 """
 import torch
 
@@ -62,6 +65,18 @@ class GraphedDetector:
     def overflow_boxes(self):
         return self.model.overflow_boxes
 
+    @property
+    def transformer(self):
+        return self.model.transformer
+
+    @property
+    def generate_attention_maps(self):
+        return bool(getattr(self.model, "generate_attention_maps", False))
+
+    @generate_attention_maps.setter
+    def generate_attention_maps(self, on):
+        self.model.generate_attention_maps = bool(on)
+
     def parameters(self):
         return self.model.parameters()
 
@@ -82,6 +97,7 @@ class GraphedDetector:
         with torch.no_grad():
             out, _, plan.features, plan.memory, plan.hs_all = forward(plan.img, targets, plan.prev)
         plan.logits, plan.out_boxes, plan.hs_embed = out["pred_logits"], out["pred_boxes"], out["hs_embed"]
+        plan.attention_maps = out.get("attention_maps")
 
     def _build(self, key, img, kb, prev_features):
         dev = img.device
@@ -129,7 +145,7 @@ class GraphedDetector:
             k = int(targets[0]["track_query_boxes"].shape[0])
         kb = self._padded_count(k)
         use_prev = self.uses_prev and prev_features is not None
-        key = (tuple(samples.shape), samples.dtype, kb, use_prev)
+        key = (tuple(samples.shape), samples.dtype, kb, use_prev, self.generate_attention_maps)
         plan = self._plans.get(key)
         if plan is None:
             plan = self._build(key, samples, kb, prev_features if use_prev else None)
@@ -159,6 +175,8 @@ class GraphedDetector:
 
         out = {"pred_logits": real_rows(plan.logits, 1), "pred_boxes": real_rows(plan.out_boxes, 1),
                "hs_embed": real_rows(plan.hs_embed, 1)}
+        if plan.attention_maps is not None:
+            out["attention_maps"] = real_rows(plan.attention_maps, 1)
         features = plan.features
         if self.uses_prev and plan.graph is not None:
             # the static feature maps are overwritten by the next replay, but the tracker hands them back as

@@ -31,6 +31,14 @@ which stays on the device.  `results[id][frame]["mask"]` is the reference's bool
 map by csrc/mask_rle.cu so that only the strings are read back (`mots.decode` gives the array); `Track.mask` is the
 frame's resolved bool mask for active tracks and None for inactive ones (the reference keeps an inactive track's last
 mask, which nothing reads: a track that comes back always takes a new one).
+
+Attention maps (`generate_attention_maps=True`, tracker.py:37-60, 335-481, 539-541; vanilla DETR models only, as in the
+reference).  The detector's `generate_attention_maps` switch makes its forward return `out["attention_maps"]`
+[1, Q, h, w], the last decoder layer's cross-attention weights averaged over heads.  A track takes a new map exactly
+where it takes a new embedding (`hs_writes`), else keeps the one it had; after the decisions the maps of the result
+rows are gathered on the device and read back in one copy.  `results[id][frame]["attention_map"]` is that float32
+[h, w] array; `Track.attention_map` is the frame's map (a host tensor) for active tracks and None for inactive ones,
+like `Track.mask`.
 """
 from collections import deque
 
@@ -120,7 +128,7 @@ class Track:
         self.hs_embed = [tracker._embedding_of(slot)]
         self.gt_id = None
         self.mask = tracker._mask_of(slot)
-        self.attention_map = None
+        self.attention_map = tracker._attention_map_of(slot)
 
     def has_positive_area(self) -> bool:
         return bool(self.pos[2] > self.pos[0] and self.pos[3] > self.pos[1])
@@ -171,11 +179,16 @@ class Tracker:
         self.prev_frame_dist = tracker_cfg["prev_frame_dist"]
         self.steps_termination = tracker_cfg["steps_termination"]
         if generate_attention_maps:
-            # the reference asserts the same for the deformable model (tracker.py:38)
-            raise ValueError("Generation of attention maps not possible for deformable DETR.")
+            # the reference asserts the same (tracker.py:38): only a vanilla decoder has a multihead_attn to read
+            layers = getattr(getattr(getattr(obj_detector, "transformer", None), "decoder", None), "layers", None)
+            if not layers or not hasattr(layers[-1], "multihead_attn"):
+                raise ValueError("Generation of attention maps not possible for deformable DETR.")
+        if hasattr(obj_detector, "generate_attention_maps"):
+            # the detector's switch follows the tracker that drives it: one built without maps turns it back off
+            obj_detector.generate_attention_maps = bool(generate_attention_maps)
         self.masks = "segm" in obj_detector_post
         self.mask_rle = bool(mask_rle)        # results' "mask": COCO RLE dicts (mots.label_map_rle) instead of bool arrays
-        self.generate_attention_maps = False
+        self.generate_attention_maps = bool(generate_attention_maps)
         self._logger = logger if logger is not None else (lambda *log_strs: None)
         self._verbose = verbose
         self._pinned = None
@@ -204,6 +217,7 @@ class Tracker:
     def reset(self, hard=True):
         """tracker.py:71-80"""
         self._label = None                    # [H, W] int32 device label map of the last frame's masks
+        self._maps = {}                       # track id -> float32 [h, w] attention map, for the last frame's results
         self._state = _State()
         self._hs = None                       # [capacity, hidden] device embeddings, allocated at the first detection
         self._active, self._inactive = [], []
@@ -218,6 +232,32 @@ class Tracker:
     # ------------------------------------------------------------------------------------------------- internals
     def _embedding_of(self, slot):
         return self._hs[slot] if self._hs is not None else None
+
+    def _attention_map_of(self, slot):
+        if slot not in self._active:
+            return None
+        m = self._maps.get(int(self._state.ids[slot]))
+        return None if m is None else torch.from_numpy(m)
+
+    def _attention_maps(self, det_out, src_rows, ids):
+        """This frame's maps of the result tracks (ids, in order): `src_rows[t]` is the query row whose map track t
+        takes, -1 to keep its previous one.  The new rows are gathered on the device and read back in one copy."""
+        maps = det_out[0]["attention_maps"][0]
+        fresh = [k for k, r in enumerate(src_rows) if r >= 0]
+        host = None
+        if fresh:
+            rows = torch.as_tensor([int(src_rows[k]) for k in fresh], dtype=torch.long).to(maps.device)
+            host = maps.index_select(0, rows).float().cpu().numpy()
+        new, j = {}, 0
+        for k, tid in enumerate(ids):
+            tid = int(tid)
+            if src_rows[k] >= 0:
+                new[tid] = host[j]
+                j += 1
+            elif tid in self._maps:
+                new[tid] = self._maps[tid]
+        self._maps = new
+        return [new.get(int(tid)) for tid in ids]
 
     def _mask_of(self, slot):
         if self._label is None or slot not in self._active:
@@ -538,14 +578,18 @@ class Tracker:
 
         # ---- masks (tracker.py:509-521) and results (tracker.py:533-548)
         self._result_rows = np.asarray([hs_writes.get(s, -1) for s in self._active], np.int64)
-        masks = None
+        masks = maps = None
         if self.masks:
             masks = self._resolve_masks(det_out, self._result_rows, st.ids[self._active], blob, (height, width))
+        if self.generate_attention_maps:
+            maps = self._attention_maps(det_out, self._result_rows, st.ids[self._active])
         for k, s in enumerate(self._active):
             box = st.pos[s] if self.obj_detector.overflow_boxes else _clip(st.pos[s], height, width)
             entry = {"bbox": box.copy(), "score": np.array(st.score[s]), "obj_ind": int(st.obj_ind[s])}
             if masks is not None:
                 entry["mask"] = masks[k]
+            if maps is not None and maps[k] is not None:
+                entry["attention_map"] = maps[k].copy()
             self.results.setdefault(int(st.ids[s]), {})[self.frame_index] = entry
         for s in self._inactive:
             st.count_inactive[s] += 1

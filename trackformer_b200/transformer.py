@@ -16,6 +16,11 @@ query), the key padding of the decoder's query self-attention.  Filler track que
 are hidden from the real queries as keys, and every other decoder op is row-wise, so the real rows are unaffected.
 ``track_attention=True`` (the reference's separate track-query self-attention, which hard-codes 100 object queries) is
 not built.
+
+``need_weights=True`` (``Transformer.forward``, ``TransformerDecoder.forward``) asks the LAST decoder layer's
+cross-attention for its weights averaged over heads -- what the reference's tracker hooks out of
+``decoder.layers[-1].multihead_attn`` for ``generate_attention_maps`` -- and ``Transformer.forward`` returns them as a
+fourth value, ``[B, Q, h, w]`` on the memory grid.  Off (the default), nothing is computed and the return is unchanged.
 """
 from __future__ import annotations
 
@@ -76,9 +81,11 @@ class Transformer(nn.Module):
         self.d_model = d_model
         self.nhead = nhead
 
-    def forward(self, src, mask, query_embed, pos_embed, tgt=None, prev_frame=None, tgt_key_padding_mask=None):
+    def forward(self, src, mask, query_embed, pos_embed, tgt=None, prev_frame=None, tgt_key_padding_mask=None,
+                need_weights=False):
         """src [B, C, h, w], mask [B, h, w], query_embed [Q, B, C], pos_embed [B, C, h, w], tgt [Q, B, C] or None
-        -> (hs [layers, B, Q, C], hs_without_norm [layers, B, Q, C], memory [B, C, h, w])."""
+        -> (hs [layers, B, Q, C], hs_without_norm [layers, B, Q, C], memory [B, C, h, w]), and with ``need_weights``
+        the last decoder layer's head-averaged cross-attention weights [B, Q, h, w] as a fourth value."""
         if prev_frame is not None:
             raise NotImplementedError("prev_frame is only used by track_attention, which is not supported")
         if self.training and src.is_cuda:
@@ -90,9 +97,13 @@ class Transformer(nn.Module):
         if tgt is None:
             tgt = torch.zeros_like(query_embed)
         memory = self.encoder(src, src_key_padding_mask=mask, pos=pos_embed)
-        hs, hs_without_norm = self.decoder(tgt, memory, tgt_key_padding_mask=tgt_key_padding_mask,
-                                           memory_key_padding_mask=mask, pos=pos_embed, query_pos=query_embed)
-        return hs.transpose(1, 2), hs_without_norm.transpose(1, 2), memory.permute(1, 2, 0).view(bs, c, h, w)
+        dec = self.decoder(tgt, memory, tgt_key_padding_mask=tgt_key_padding_mask, memory_key_padding_mask=mask,
+                           pos=pos_embed, query_pos=query_embed, need_weights=need_weights)
+        hs, hs_without_norm = dec[0], dec[1]
+        res = hs.transpose(1, 2), hs_without_norm.transpose(1, 2), memory.permute(1, 2, 0).view(bs, c, h, w)
+        if need_weights:
+            return res + (dec[2].view(bs, -1, h, w),)
+        return res
 
 
 class TransformerEncoder(nn.Module):
@@ -127,21 +138,25 @@ class TransformerDecoder(nn.Module):
         self.track_attention = False
 
     def forward(self, tgt, memory, tgt_mask=None, memory_mask=None, tgt_key_padding_mask=None,
-                memory_key_padding_mask=None, pos=None, query_pos=None):
+                memory_key_padding_mask=None, pos=None, query_pos=None, need_weights=False):
+        """-> (output, output without the final norm), plus the last layer's head-averaged cross-attention weights
+        [B, Q, Lk] when ``need_weights``."""
         if tgt_mask is not None or memory_mask is not None:
             raise NotImplementedError("attention masks other than key padding are not supported")
         output = tgt
         intermediate = []
-        for layer in self.layers:
+        for i, layer in enumerate(self.layers):
             output = layer(output, memory, tgt_key_padding_mask=tgt_key_padding_mask,
-                           memory_key_padding_mask=memory_key_padding_mask, pos=pos, query_pos=query_pos)
+                           memory_key_padding_mask=memory_key_padding_mask, pos=pos, query_pos=query_pos,
+                           need_weights=need_weights and i + 1 == len(self.layers))
+            if need_weights and i + 1 == len(self.layers):
+                output, weights = output
             if self.return_intermediate:
                 intermediate.append(output)
         if self.return_intermediate:
             output = torch.stack(intermediate)
-        if self.norm is not None:
-            return self.norm(output), output
-        return output, output
+        res = (self.norm(output), output) if self.norm is not None else (output, output)
+        return res + (weights,) if need_weights else res
 
 
 class TransformerEncoderLayer(nn.Module):
@@ -202,32 +217,42 @@ class TransformerDecoderLayer(nn.Module):
     with_pos_embed = staticmethod(_add_pos)
 
     def forward_post(self, tgt, memory, tgt_key_padding_mask=None, memory_key_padding_mask=None, pos=None,
-                     query_pos=None):
+                     query_pos=None, need_weights=False):
         tgt2 = _self_attention(self.self_attn, _add_pos(tgt, query_pos), tgt, tgt_key_padding_mask)
         tgt = add_dropout_layernorm(tgt, tgt2, self.dropout1, self.norm1)
         tgt2 = dense_attention.attention(self.multihead_attn, _add_pos(tgt, query_pos), _add_pos(memory, pos), memory,
-                                         memory_key_padding_mask)
+                                         memory_key_padding_mask, need_weights)
+        if need_weights:
+            tgt2, weights = tgt2
         tgt = add_dropout_layernorm(tgt, tgt2, self.dropout2, self.norm2)
         tgt2 = _ffn(tgt, self.linear1, self.linear2, self.activation, self.dropout)
-        return add_dropout_layernorm(tgt, tgt2, self.dropout3, self.norm3)
+        tgt = add_dropout_layernorm(tgt, tgt2, self.dropout3, self.norm3)
+        return (tgt, weights) if need_weights else tgt
 
     def forward_pre(self, tgt, memory, tgt_key_padding_mask=None, memory_key_padding_mask=None, pos=None,
-                    query_pos=None):
+                    query_pos=None, need_weights=False):
         tgt2 = self.norm1(tgt)
         tgt = tgt + self.dropout1(_self_attention(self.self_attn, _add_pos(tgt2, query_pos), tgt2, tgt_key_padding_mask))
         tgt2 = self.norm2(tgt)
-        tgt = tgt + self.dropout2(dense_attention.attention(self.multihead_attn, _add_pos(tgt2, query_pos),
-                                                            _add_pos(memory, pos), memory, memory_key_padding_mask))
+        tgt2 = dense_attention.attention(self.multihead_attn, _add_pos(tgt2, query_pos), _add_pos(memory, pos), memory,
+                                         memory_key_padding_mask, need_weights)
+        if need_weights:
+            tgt2, weights = tgt2
+        tgt = tgt + self.dropout2(tgt2)
         tgt2 = _ffn(self.norm3(tgt), self.linear1, self.linear2, self.activation, self.dropout)
-        return tgt + self.dropout3(tgt2)
+        tgt = tgt + self.dropout3(tgt2)
+        return (tgt, weights) if need_weights else tgt
 
     def forward(self, tgt, memory, tgt_mask=None, memory_mask=None, tgt_key_padding_mask=None,
-                memory_key_padding_mask=None, pos=None, query_pos=None):
+                memory_key_padding_mask=None, pos=None, query_pos=None, need_weights=False):
+        """-> tgt, or ``(tgt, cross-attention weights averaged over heads [B, Q, Lk])`` with ``need_weights``."""
         if tgt_mask is not None or memory_mask is not None:
             raise NotImplementedError("attention masks other than key padding are not supported")
         if self.normalize_before:
-            return self.forward_pre(tgt, memory, tgt_key_padding_mask, memory_key_padding_mask, pos, query_pos)
-        return self.forward_post(tgt, memory, tgt_key_padding_mask, memory_key_padding_mask, pos, query_pos)
+            return self.forward_pre(tgt, memory, tgt_key_padding_mask, memory_key_padding_mask, pos, query_pos,
+                                    need_weights)
+        return self.forward_post(tgt, memory, tgt_key_padding_mask, memory_key_padding_mask, pos, query_pos,
+                                 need_weights)
 
 
 def build_transformer(args):
