@@ -309,6 +309,13 @@ typedef struct TfbTrackStepArgs {
 
 int tfb200_track_step_f32(const TfbTrackStepArgs* args, void* stream);
 
+/* n independent sequences in ONE launch of n CTAs: CTA b takes every decision of tfb200_track_step_f32 on args[b]
+ * (its own state, scratch, result buffer, public detections and thresholds), so the results are those of n single
+ * calls.  The n structs are passed by value (kernel parameter space), so the launch reads no host memory and can be
+ * captured in a CUDA graph.  n must be 1..16, else TFB200_E_SHAPE; any invalid args[b] returns what
+ * tfb200_track_step_f32 returns for it.  On an error nothing is launched.                                          */
+int tfb200_track_step_batched_f32(const TfbTrackStepArgs* args, int n, void* stream);
+
 /* Segmentation mask head between its convolutions, and its loss (csrc/mask_head.cu; reference
  * models/detr_segmentation.py:111-216, models/detr.py:330-357).  Per-query maps are channels-last [N][HW][C] with
  * N = images * per_image; an operand "per image" is [N / per_image][...] and is broadcast over that image's queries

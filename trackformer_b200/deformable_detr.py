@@ -75,9 +75,10 @@ class DETR(nn.Module):
     def _set_aux_loss(self, outputs_class, outputs_coord):
         return [{"pred_logits": a, "pred_boxes": b} for a, b in zip(outputs_class[:-1], outputs_coord[:-1])]
 
-    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None):
+    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None, prev_valid=None):
         """Vanilla DETR (detr.py:62-128): single-level ``input_proj``, track queries as zero ``query_embed`` rows whose
-        decoder input is ``track_query_hs_embeds``.  ``prev_features`` is accepted (the tracker passes it) and ignored:
+        decoder input is ``track_query_hs_embeds``.  ``prev_features`` and ``prev_valid`` are accepted (the trackers
+        pass them) and ignored:
         vanilla DETR has no multi-frame path.  ``track_query_padding`` [K] per image marks filler track queries, hidden
         from the others as self-attention keys (GraphedDetector, TrainStep).  Unlike the reference, the targets'
         ``track_query_hs_embeds`` are not overwritten with the full decoder input rows.  With
@@ -225,13 +226,23 @@ class DeformableDETR(DETR):
         """(logits [layers, N, Q, classes], boxes [layers, N, Q, 4]) of the latest forward call, or None"""
         return self._call_scratch().value
 
-    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None):
+    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None, prev_valid=None):
+        """``prev_valid`` [B] bool (optional, with ``prev_features``): where False, image b has no previous frame and
+        its own features stand in for ``prev_features`` -- as a whole call with ``prev_features=None`` does.  The select
+        runs on the device, so a CUDA graph can take the flags as a static input."""
         self._call_scratch().value = None                # do not keep the previous call's graph alive
         if not isinstance(samples, NestedTensor):
             samples = nested_tensor_from_tensor_list(samples)
         features_all, pos = self.backbone(samples)
         features = features_all[-3:]
-        prev_features = features if prev_features is None else prev_features[-3:]
+        if prev_features is None:
+            prev_features = features
+        elif prev_valid is None:
+            prev_features = prev_features[-3:]
+        else:
+            keep = prev_valid.view(-1, 1, 1, 1)
+            prev_features = [NestedTensor(torch.where(keep, p.tensors, f.tensors), p.mask)
+                             for p, f in zip(prev_features[-3:], features)]
 
         src_list, mask_list, pos_list = [], [], []
         frames = [prev_features, features] if self.multi_frame_attention else [features]

@@ -107,7 +107,7 @@ class DETRTrackingBase(nn.Module):
             target["track_queries_fal_pos_mask"] = torch.cat([~still_there, pad]).to(device)
 
     # ------------------------------------------------------------------------------------------
-    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None):
+    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None, prev_valid=None):
         if targets is not None and not self._tracking:
             prev_targets = [t["prev_target"] for t in targets]
             if self.training:
@@ -137,7 +137,7 @@ class DETRTrackingBase(nn.Module):
                     t["track_queries_fal_pos_mask"] = torch.zeros(self.num_queries).bool().to(dev)
                     t["track_query_boxes"] = torch.zeros(0, 4).to(dev)
                     t["track_query_match_ids"] = torch.tensor([]).long().to(dev)
-        return super().forward(samples, targets, prev_features)
+        return super().forward(samples, targets, prev_features, prev_valid)
 
 
 class DeformableDETRTracking(DETRTrackingBase, DeformableDETR):

@@ -185,37 +185,11 @@ class DeviceTracker(Tracker):
         nq = self.num_object_queries
         assert rows.shape[0] == n_query + nq, (rows.shape, n_query, nq)
 
-        public = None
-        if self.public_detections:
-            public = blob["dets"][0] if "dets" in blob else []
-            public = torch.as_tensor(np.asarray(public.cpu() if torch.is_tensor(public) else public, dtype=np.float32)
-                                     .reshape(-1, 4)).to(dev)
+        public = self._public(blob, dev)
         n_public = 0 if public is None else int(public.shape[0])
         self._ensure(hs_embeds.shape[1], nq, n_public, dev)
         b = self._bufs
-        src, dst = b["state"][self._cur], b["state"][1 - self._cur]
-
-        a = _ArgsC()
-        a.rows, a.hs_embeds = rows.data_ptr(), hs_embeds.data_ptr()
-        a.public_dets = public.data_ptr() if n_public else None
-        for c_state, t_state in ((a.inp, src), (a.out, dst)):
-            for name in t_state:
-                setattr(c_state, name, t_state[name].data_ptr())
-        for name in ("q_boxes", "q_embeds", "result", "iscratch", "fscratch", "dscratch"):
-            setattr(a, name, b[name].data_ptr())
-        a.inactive_patience, a.reid_sim_threshold = float(self.inactive_patience), float(self.reid_sim_threshold)
-        a.detection_obj_score_thresh = float(self.detection_obj_score_thresh)
-        a.track_obj_score_thresh = float(self.track_obj_score_thresh)
-        a.reid_score_thresh = float(self.reid_score_thresh)
-        a.detection_nms_thresh = float(self.detection_nms_thresh or 0.0)
-        a.track_nms_thresh = float(self.track_nms_thresh or 0.0)
-        a.capacity, a.hidden, a.nq, a.n_query, a.n_public = b["capacity"], b["hidden"], nq, n_query, n_public
-        a.img_h, a.img_w = height, width
-        a.overflow_boxes = int(bool(self.obj_detector.overflow_boxes))
-        a.public_mode = _PUBLIC_MODES[self.public_detections]
-        a.reid_greedy_matching, a.reid_sim_only = int(bool(self.reid_greedy_matching)), int(bool(self.reid_sim_only))
-        a.steps_termination = int(self.steps_termination)
-        a.detection_nms_on, a.track_nms_on = int(bool(self.detection_nms_thresh)), int(bool(self.track_nms_thresh))
+        a = self._args(rows.data_ptr(), hs_embeds.data_ptr(), public, b["result"].data_ptr(), nq, height, width)
         tensors = [rows, hs_embeds, b["result"]] + ([public] if n_public else [])
         self._launch(a, tensors)
 
@@ -225,7 +199,48 @@ class DeviceTracker(Tracker):
         host.copy_(b["result"][:words], non_blocking=True)
         if host.is_pinned():
             torch.cuda.current_stream(dev).synchronize()
-        out = host.numpy()
+        self._take_results(host.numpy(), det_out, blob, height, width)
+        self._prev_features.append(features)
+
+    def _public(self, blob, dev):
+        """This frame's public detections [n, 4] on the device (None when the tracker does not use them)."""
+        if not self.public_detections:
+            return None
+        public = blob["dets"][0] if "dets" in blob else []
+        return torch.as_tensor(np.asarray(public.cpu() if torch.is_tensor(public) else public, dtype=np.float32)
+                               .reshape(-1, 4)).to(dev)
+
+    def _args(self, rows, hs_embeds, public, result, nq, height, width):
+        """The kernel's arguments for this frame (after `_ensure`): `rows` / `hs_embeds` / `result` device addresses."""
+        b = self._bufs
+        n_public = 0 if public is None else int(public.shape[0])
+        src, dst = b["state"][self._cur], b["state"][1 - self._cur]
+        a = _ArgsC()
+        a.rows, a.hs_embeds = rows, hs_embeds
+        a.public_dets = public.data_ptr() if n_public else None
+        for c_state, t_state in ((a.inp, src), (a.out, dst)):
+            for name in t_state:
+                setattr(c_state, name, t_state[name].data_ptr())
+        for name in ("q_boxes", "q_embeds", "iscratch", "fscratch", "dscratch"):
+            setattr(a, name, b[name].data_ptr())
+        a.result = result
+        a.inactive_patience, a.reid_sim_threshold = float(self.inactive_patience), float(self.reid_sim_threshold)
+        a.detection_obj_score_thresh = float(self.detection_obj_score_thresh)
+        a.track_obj_score_thresh = float(self.track_obj_score_thresh)
+        a.reid_score_thresh = float(self.reid_score_thresh)
+        a.detection_nms_thresh = float(self.detection_nms_thresh or 0.0)
+        a.track_nms_thresh = float(self.track_nms_thresh or 0.0)
+        a.capacity, a.hidden, a.nq, a.n_query, a.n_public = b["capacity"], b["hidden"], nq, self._n_query, n_public
+        a.img_h, a.img_w = height, width
+        a.overflow_boxes = int(bool(self.obj_detector.overflow_boxes))
+        a.public_mode = _PUBLIC_MODES[self.public_detections]
+        a.reid_greedy_matching, a.reid_sim_only = int(bool(self.reid_greedy_matching)), int(bool(self.reid_sim_only))
+        a.steps_termination = int(self.steps_termination)
+        a.detection_nms_on, a.track_nms_on = int(bool(self.detection_nms_thresh)), int(bool(self.track_nms_thresh))
+        return a
+
+    def _take_results(self, out, det_out, blob, height, width):
+        """Book the frame from its read-back words `out` (header + result rows) and advance to the next frame."""
         n_active, n_inactive, track_num, num_reids, n_next, error, n_results = (int(v) for v in out[:7])
         if error:
             raise RuntimeError(f"track_step kernel reported error {error} (1: query count / state mismatch, 2: capacity)")
@@ -252,7 +267,6 @@ class DeviceTracker(Tracker):
         self._cur = 1 - self._cur
         self._host_view = None
         self.frame_index += 1
-        self._prev_features.append(features)
 
     # ------------------------------------------------------------------------------------- host views (on demand)
     def _download(self):

@@ -1,7 +1,8 @@
 """CUDA-graph replay of the tracking-mode detector forward (SURVEY section 8, row f3).
 
-Online tracking is batch-1 and latency-bound: the reference issues ~2000 small kernels per frame from Python
-(src/trackformer/models/tracker.py:306 -> DeformableDETR.forward) and the number of track queries changes from frame to
+Online tracking of one sequence is batch-1 and latency-bound (`batched`, below, steps several sequences together):
+the reference issues ~2000 small kernels per frame from Python (src/trackformer/models/tracker.py:306 ->
+DeformableDETR.forward) and the number of track queries changes from frame to
 frame, so nothing about a frame's launch sequence is reusable as it stands.  `GraphedDetector` makes it reusable:
 
   * the track queries of a frame are padded up to a multiple of `bucket` with filler queries that the real queries
@@ -188,6 +189,124 @@ class GraphedDetector:
         # NB: for models that never read prev_features the returned `features` / `memory` (and, when no filler rows had
         # to be dropped, the output rows) are views of the graph's static buffers: valid until the next call.
         return out, targets, features, plan.memory, real_rows(plan.hs_all, 2)
+
+    def _build_batched(self, samples, kb, prev_features):
+        dev, bsz = samples.device, samples.shape[0]
+        plan = _Plan()
+        plan.kb = kb
+        plan.img = samples.clone()
+        if kb:
+            plan.hs = torch.zeros(bsz, kb, self.hidden_dim, device=dev)
+            plan.boxes = torch.full((bsz, kb, 4), 0.5, device=dev)
+            plan.padding = torch.ones(bsz, kb, dtype=torch.bool, device=dev)
+            plan.slot_index = torch.arange(kb, device=dev)
+            plan.first = torch.zeros(bsz, 1, dtype=torch.int64, device=dev)
+            plan.image_id = torch.tensor([1], device=dev)
+        if prev_features is not None:
+            plan.prev_valid = torch.zeros(bsz, dtype=torch.bool, device=dev)
+            src, i = next(p for p in prev_features if p is not None)
+            plan.prev = []
+            for f in src:
+                mask = f.mask[i:i + 1].expand(bsz, -1, -1).clone()
+                if getattr(f.mask, "_no_padding", False):
+                    mask._no_padding = True
+                plan.prev.append(NestedTensor(f.tensors[i:i + 1].repeat(bsz, 1, 1, 1), mask))
+        plan.graph = None
+        if self.use_graphs:
+            if not samples.is_cuda:
+                raise RuntimeError("GraphedDetector(use_graphs=True) needs CUDA tensors")
+            if hasattr(self.model.backbone[0], "prepare"):
+                self.model.backbone[0].prepare()
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                for _ in range(self.warmup):
+                    self._run_batched(plan)
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            plan.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(plan.graph):
+                self._run_batched(plan)
+            self.captures += 1
+        return plan
+
+    def _run_batched(self, plan):
+        targets = None
+        if plan.kb:
+            targets = [{"track_query_boxes": plan.boxes[b], "track_query_hs_embeds": plan.hs[b],
+                        "track_query_padding": plan.padding[b], "image_id": plan.image_id}
+                       for b in range(plan.img.shape[0])]
+        forward = self.model.detect if self.has_mask_head else self.model
+        prev_valid = None if plan.prev is None else plan.prev_valid
+        with torch.no_grad():
+            out, _, features, _, _ = forward(plan.img, targets, plan.prev, prev_valid)
+        plan.features = features[-3:]
+        plan.logits, plan.out_boxes, plan.hs_embed = out["pred_logits"], out["pred_boxes"], out["hs_embed"]
+
+    def batched(self, samples, targets=None, prev_features=None):
+        """One forward of B images that each carry their own track queries -- B independent sequences stepped together.
+
+        ``samples`` [B, 3, H, W] (one input size: images of different sizes would be padded, which changes the border
+        sampling of a batch-1 run).  ``targets[b]`` holds image b's ``track_query_boxes`` [K_b, 4] and
+        ``track_query_hs_embeds`` [K_b, C] (or is None: K_b = 0).  ``prev_features[b]`` is ``(features, i)`` -- image i
+        of a ``features`` list this method returned earlier -- or None where the image has no previous frame; the
+        model then reads the image's own features, as a batch-1 call with ``prev_features=None`` does.
+
+        All images are padded to ``kb`` = the bucket of max K_b track queries.  Image b's K_b track queries take the
+        LAST K_b of its kb slots, so its real rows ``[kb - K_b, kb + nq)`` (track queries, then object queries) are
+        contiguous and a consumer reads them in place with a row offset.  One CUDA graph is captured per (B, H, W,
+        dtype, kb, previous-frame features yes/no); which images have a previous frame is a static input of it.
+
+        Returns ``(out, features, ks, kb)``: ``out`` with the padded ``pred_logits`` / ``pred_boxes`` / ``hs_embed``
+        [B, kb + nq, .] (views of the graph's buffers: valid until the next call), the levels ``features`` a later
+        call takes as ``prev_features`` (its own copy), and the host ints K_b."""
+        if not torch.is_tensor(samples) or samples.ndim != 4:
+            raise ValueError("GraphedDetector.batched takes one [B, 3, H, W] tensor of same-sized images")
+        bsz = samples.shape[0]
+        targets = [None] * bsz if targets is None else list(targets)
+        prev_features = [None] * bsz if prev_features is None else list(prev_features)
+        if len(targets) != bsz or len(prev_features) != bsz:
+            raise ValueError("GraphedDetector.batched: one target and one prev_features entry per image")
+        ks = [0 if t is None else int(t["track_query_boxes"].shape[0]) for t in targets]
+        kb = self._padded_count(max(ks))
+        use_prev = self.uses_prev and any(p is not None for p in prev_features)
+        key = ("batched", tuple(samples.shape), samples.dtype, kb, use_prev, self.generate_attention_maps)
+        plan = self._plans.get(key)
+        if plan is None:
+            plan = self._plans[key] = self._build_batched(samples, kb, prev_features if use_prev else None)
+        self._last = None
+        plan.img.copy_(samples, non_blocking=True)
+        if kb:
+            for b, (t, k) in enumerate(zip(targets, ks)):
+                if k:
+                    plan.hs[b, kb - k:].copy_(t["track_query_hs_embeds"], non_blocking=True)
+                    plan.boxes[b, kb - k:].copy_(t["track_query_boxes"], non_blocking=True)
+            plan.first.copy_(torch.tensor([[kb - k] for k in ks]), non_blocking=True)
+            torch.lt(plan.slot_index, plan.first, out=plan.padding)
+        if use_prev:
+            valid = [p is not None for p in prev_features]
+            plan.prev_valid.copy_(torch.tensor(valid), non_blocking=True)
+            src = {id(p[0]) for p in prev_features if p is not None}
+            whole = (all(valid) and len(src) == 1 and all(p[1] == b for b, p in enumerate(prev_features))
+                     and prev_features[0][0][0].tensors.shape[0] == bsz)
+            if whole:                                     # the batch of the last step, in the same order
+                for dst, f in zip(plan.prev, prev_features[0][0]):
+                    dst.tensors.copy_(f.tensors, non_blocking=True)
+            else:
+                for b, p in enumerate(prev_features):
+                    if p is not None:
+                        for dst, f in zip(plan.prev, p[0]):
+                            dst.tensors[b].copy_(f.tensors[p[1]], non_blocking=True)
+        if plan.graph is not None:
+            plan.graph.replay()
+            self.replays += 1
+        else:
+            self._run_batched(plan)
+        features = plan.features
+        if self.uses_prev and plan.graph is not None:
+            features = [NestedTensor(f.tensors.clone(), f.mask) for f in plan.features]
+        out = {"pred_logits": plan.logits, "pred_boxes": plan.out_boxes, "hs_embed": plan.hs_embed}
+        return out, features, ks, kb
 
     def detect(self, samples, targets=None, prev_features=None):
         """The call itself: for segmentation models the graph already holds the forward without the mask head."""

@@ -335,14 +335,14 @@ class DETRSegmBase(nn.Module):
         self.bbox_attention = MHAttentionMap(self.hidden_dim, self.hidden_dim, nheads, dropout=0.0)
         self.mask_head = MaskHeadSmallConv(self.hidden_dim + nheads, self.fpn_channels, self.hidden_dim)
 
-    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None):
-        out, targets, features, memory, hs = self.detect(samples, targets, prev_features)
+    def forward(self, samples: NestedTensor, targets: list = None, prev_features=None, prev_valid=None):
+        out, targets, features, memory, hs = self.detect(samples, targets, prev_features, prev_valid)
         out["pred_masks"] = self.mask_logits(features, memory, hs)
         return out, targets, features, memory, hs
 
-    def detect(self, samples: NestedTensor, targets: list = None, prev_features=None):
+    def detect(self, samples: NestedTensor, targets: list = None, prev_features=None, prev_valid=None):
         """The detection forward without the mask head: ``forward``'s return value without ``pred_masks``."""
-        return super().forward(samples, targets, prev_features)
+        return super().forward(samples, targets, prev_features, prev_valid)
 
     def mask_logits(self, features, memory, hs, rows=None) -> Tensor:
         """Mask logits ``[B, len(rows), H/4, W/4]`` of the query rows ``rows`` (all rows if None) from the outputs of
