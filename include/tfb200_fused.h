@@ -411,6 +411,31 @@ int64_t tfb200_mask_rle_max_bytes(int H, int W, int T);
 int tfb200_mask_rle_i32(const int32_t* label, const int32_t* ids, int H, int W, int T, void* workspace,
                         size_t workspace_bytes, int64_t* header, char* chars, int64_t chars_capacity, void* stream);
 
+/* MOTChallenge CLEAR-MOT and identity metrics of S sequences at once (csrc/mot_eval.cu; what motmetrics 1.2.0
+ * computes for get_mot_accum / evaluate_mot_accums, src/trackformer/util/track_utils.py:354-417).  F frames over all
+ * sequences in order; frame f holds object rows frame_obj[f] .. frame_obj[f + 1] and hypothesis rows frame_hyp[f] ..
+ * frame_hyp[f + 1] (int32 [F + 1], non-decreasing, from 0), in the order motmetrics is given them.  obj_id / hyp_id:
+ * the row's dense GT / track id within its sequence; obj_box / hyp_box [rows][4] float32 x, y, w, h.  seq [S][8]
+ * int64 = {frame begin, frame end, GT-id begin, GT-id count, track-id begin, track-id count, tp-cell begin, 0}: the
+ * GT ids of sequence s are n_gt's entries from its begin (likewise tracks), its tp matrix [GT-id count][track-id
+ * count] int32 starts at its tp-cell begin of tp_cells.  A pair is valid when 1 - IoU <= 0.5 (fp64 IoU of the boxes
+ * extended to x + w, y + h).  Writes out [S][16] 8-byte slots = {status, valid pairs, matches, switches, misses, false
+ * positives, fragmentations, mostly tracked, partially tracked, mostly lost, IDTP, largest residual component of a
+ * frame (objects, hypotheses), largest identity component (GT ids, track ids), sum of d over matches and switches as
+ * a double}.  status bit 1: more than pair_cap valid pairs (slot 1 holds the count; nothing past the pairs is
+ * computed: call again with pair_cap >= the sum of slot 1); bit 2: a frame with more than max_obj objects or max_hyp
+ * hypotheses; bit 4: a residual component over 64 objects or 64 hypotheses; bit 8: an identity component whose
+ * smaller side (GT ids or track ids) is over 8192 or larger side over 65536.  A set bit leaves that sequence's counts
+ * incomplete.  Workspace: tfb200_mot_eval_workspace_bytes(...) bytes (0 for bad sizes), about 16 B per pair of
+ * pair_cap plus 4 B per tp cell.  Integer counts are exact and every output is the same run to run.  Sizes out of
+ * range: TFB200_E_SHAPE.                                                                                           */
+size_t tfb200_mot_eval_workspace_bytes(int S, int F, int64_t n_gt, int64_t n_trk, int64_t tp_cells, int max_obj,
+                                       int max_hyp, int64_t pair_cap);
+int tfb200_mot_eval_f32(const int64_t* seq, const int32_t* frame_obj, const int32_t* frame_hyp, const int32_t* obj_id,
+                        const float* obj_box, const int32_t* hyp_id, const float* hyp_box, int S, int F, int64_t n_gt,
+                        int64_t n_trk, int64_t tp_cells, int max_obj, int max_hyp, int64_t pair_cap, void* workspace,
+                        size_t workspace_bytes, int64_t* out, void* stream);
+
 /* Frame ingest (csrc/frame_ingest.cu; reference: the per-frame host work of datasets/tracking/mot17_sequence.py:68-81,
  * i.e. Pillow's bilinear resize of the 8-bit image, to_tensor and Normalize): src [H][W][3] interleaved uint8 with
  * src_row_stride bytes between rows (>= 3 * W)  ->  dst[c * dst_plane_stride + y * dst_row_stride + x] fp32, c < 3,
