@@ -436,6 +436,48 @@ int tfb200_mot_eval_f32(const int64_t* seq, const int32_t* frame_obj, const int3
                         int64_t n_trk, int64_t tp_cells, int max_obj, int max_hyp, int64_t pair_cap, void* workspace,
                         size_t workspace_bytes, int64_t* out, void* stream);
 
+/* COCO box / mask AP (csrc/coco_eval.cu; what pycocotools 2.0's COCOeval computes for the reference's CocoEvaluator,
+ * datasets/coco_eval.py).  tfb200_coco_match_f32 evaluates the B images of one update.  img [B][10] int64 = {GT image
+ * row, first detection row, detection count, H, W, device address of the image's masks uint8/bool [n][H][W] (segm),
+ * IoU-matrix offset (cells), detection bit-plane offset (words), GT bit-plane offset (words), matched-flag offset
+ * (bytes)}, the offsets laid out by the caller (per image n x G IoU cells, n x W x ceil(H / 32) and G x W x ceil(H / 32)
+ * words, A x T x G bytes, G = the image's GT rows); max_n / max_g the largest n / G.  boxes [N][4] float32 x0, y0,
+ * x1, y1, scores [N] float32, labels [N] int64 (category id = label + 1), cat_ids [K] ascending.  Ground truth of the
+ * whole dataset: gt_off [images + 1], per row (sorted by category index within an image, JSON order otherwise) gt_k,
+ * gt_box [4] x, y, w, h fp64, gt_area fp64, gt_crowd, gt_id int64; segm: gt_run_off / gt_runs [runs][2] (column-major
+ * start, length of each run of ones), gt_bbox [4] int32 inclusive tight box, gt_px pixel count.  area_rng [A][2],
+ * iou_thr [T] (min(t, 1 - 1e-10)), max_det (maxDets[-1]).  Writes per detection the sort key ((category index << 32)
+ * | descending-score bits, K << 32 when it is not evaluated), its rank within (image, category) and state [N][A]
+ * 2 bits per threshold (0 false positive, 1 true positive, 2 ignored), and ors 1 into status for a non-finite score.
+ * Limits: n <= TFB200_COCO_MAX_DETS detections per image (TFB200_E_SHAPE beyond), A <= 8, T <= 16; the evaluator
+ * also keeps an image's ground truths of one category <= TFB200_COCO_MAX_GT.  Sizes out of range: TFB200_E_SHAPE.
+ * tfb200_coco_accumulate_f32 runs accumulate over the records of all updates (key, rank, state as written above,
+ * n_rec rows): kept [n_kept][3] = {record begin, destination begin, count} of every evaluated image in image-id order
+ * (n = the sum of counts), npig [K][A] non-ignored GT counts, rec_thr [R] (R <= 1024), max_dets [M] (M <= 8).  Writes
+ * precision / scores [T][R][K][A][M] and recall [T][K][A][M] fp64 (-1 where npig is 0), and status_out = status.
+ * Deterministic.  Workspaces: the *_workspace_bytes queries (0 for bad sizes), 256-byte aligned.  The match
+ * workspace is laid out for every detection and ground truth of each image (the caller cannot know which detections
+ * rank within the first max_det of their category without reading the scores back): 8 B per IoU cell, plus for segm
+ * 4 B x W x ceil(H / 32) per detection and per ground truth, e.g. about 78 MB for 300 detections at 1080 x 1920. */
+#define TFB200_COCO_MAX_DETS 4096
+#define TFB200_COCO_MAX_GT 4096
+size_t tfb200_coco_match_workspace_bytes(int64_t N, int64_t iou_cells, int64_t dbit_words, int64_t gbit_words,
+                                         int64_t gtm_bytes);
+int tfb200_coco_match_f32(const int64_t* img, int B, int max_n, int max_g, const float* boxes, const float* scores,
+                          const int64_t* labels, int64_t N, const int64_t* cat_ids, int K, const int64_t* gt_off,
+                          const int32_t* gt_k, const double* gt_box, const double* gt_area, const uint8_t* gt_crowd,
+                          const int64_t* gt_id, const int64_t* gt_run_off, const uint32_t* gt_runs,
+                          const int32_t* gt_bbox, const int64_t* gt_px, const double* area_rng, int A,
+                          const double* iou_thr, int T, int max_det, int segm, int64_t iou_cells, int64_t dbit_words,
+                          int64_t gbit_words, int64_t gtm_bytes, void* workspace, size_t workspace_bytes,
+                          uint64_t* key, int32_t* rank, uint32_t* state, int32_t* status, void* stream);
+size_t tfb200_coco_accumulate_workspace_bytes(int64_t n);
+int tfb200_coco_accumulate_f32(const uint64_t* key, const int32_t* rank, const uint32_t* state, int64_t n_rec,
+                               const int64_t* kept, int n_kept, int64_t n, const int64_t* npig, const double* rec_thr,
+                               const int32_t* max_dets, const int32_t* status, int K, int A, int T, int R, int M,
+                               void* workspace, size_t workspace_bytes, double* precision, double* recall,
+                               double* scores, double* status_out, void* stream);
+
 /* Frame ingest (csrc/frame_ingest.cu; reference: the per-frame host work of datasets/tracking/mot17_sequence.py:68-81,
  * i.e. Pillow's bilinear resize of the 8-bit image, to_tensor and Normalize): src [H][W][3] interleaved uint8 with
  * src_row_stride bytes between rows (>= 3 * W)  ->  dst[c * dst_plane_stride + y * dst_row_stride + x] fp32, c < 3,

@@ -13,7 +13,7 @@ import os
 import numpy as np
 import torch
 
-__all__ = ["encode", "decode", "label_map_rle", "write_results"]
+__all__ = ["encode", "decode", "decode_counts", "label_map_rle", "write_results"]
 
 _MAX_CHARS = 13                 # characters of any int64 count difference
 
@@ -56,7 +56,15 @@ def encode(mask) -> dict:
 def decode(rle: dict) -> np.ndarray:
     """bool mask [H, W] of a COCO RLE (``encode``'s inverse; pycocotools ``rleFrString`` + ``decode``)."""
     h, w = (int(v) for v in rle["size"])
-    s = rle["counts"]
+    cnts = decode_counts(rle["counts"])
+    if (cnts < 0).any() or cnts.sum() != h * w:
+        raise ValueError(f"decode: the runs do not cover a {h}x{w} mask")
+    vals = (np.arange(len(cnts)) % 2).astype(bool)
+    return np.repeat(vals, cnts).reshape(w, h).T.copy()
+
+
+def decode_counts(s) -> np.ndarray:
+    """int64 run lengths of a compressed RLE counts string (pycocotools ``rleFrString``), zero run first."""
     c = np.frombuffer(s.encode() if isinstance(s, str) else bytes(s), np.uint8).astype(np.int64) - 48
     if c.size == 0 or c[-1] & 0x20:
         raise ValueError("decode: truncated counts string")
@@ -70,10 +78,7 @@ def decode(rle: dict) -> np.ndarray:
     for first in (3, 4):                                 # cnts[i] = x[i] + cnts[i - 2] for i > 2
         if len(x) > first:
             cnts[first::2] = cnts[first - 2] + np.cumsum(x[first::2])
-    if (cnts < 0).any() or cnts.sum() != h * w:
-        raise ValueError(f"decode: the runs do not cover a {h}x{w} mask")
-    vals = (np.arange(len(cnts)) % 2).astype(bool)
-    return np.repeat(vals, cnts).reshape(w, h).T.copy()
+    return cnts
 
 
 def label_map_rle(label, ids) -> list:

@@ -462,12 +462,17 @@ class PostProcessSegm(nn.Module):
         self.threshold = threshold
 
     @torch.no_grad()
-    def forward(self, results, outputs, orig_target_sizes, max_target_sizes, return_probs=False, results_mask=None):
+    def forward(self, results, outputs, orig_target_sizes, max_target_sizes, return_probs=False, results_mask=None,
+                masks_on_device=False):
+        """`masks_on_device=True` keeps the masks where the model's outputs are, as bool (or the probabilities with
+        `return_probs`), with the values of the default route: COCO mask evaluation then reads them in place."""
         assert len(orig_target_sizes) == len(max_target_sizes)
         max_h, max_w = max_target_sizes.max(0)[0].tolist()
         outputs_masks = outputs["pred_masks"].squeeze(2)
         outputs_masks = F.interpolate(outputs_masks, size=(max_h, max_w), mode="bilinear", align_corners=False)
-        outputs_masks = outputs_masks.sigmoid().cpu()
+        outputs_masks = outputs_masks.sigmoid()
+        if not masks_on_device:
+            outputs_masks = outputs_masks.cpu()
         if not return_probs:
             outputs_masks = outputs_masks > self.threshold
 
@@ -476,7 +481,7 @@ class PostProcessSegm(nn.Module):
             masks = cur_mask[:, :img_h, :img_w].unsqueeze(1)
             masks = F.interpolate(masks.float(), size=tuple(tt.tolist()), mode="nearest")
             if not return_probs:
-                masks = masks.byte()
+                masks = masks.bool() if masks_on_device else masks.byte()
             if results_mask is not None:
                 masks = masks[results_mask[i]]
             results[i]["masks"] = masks
