@@ -397,6 +397,22 @@ int tfb200_track_masks_f32(const float* logits, const int32_t* src, const int32_
                            int32_t* label, int T, int h, int w, int size_h, int size_w, int crop_h, int crop_w, int H,
                            int W, void* stream);
 
+/* tfb200_track_masks_f32 for n images (1..16, else TFB200_E_SHAPE) in ONE launch: args[b] holds image b's arguments,
+ * each with its own logits, src, ids, prev_label, label and sizes (label sizes may differ).  Image b's label map equals
+ * tfb200_track_masks_f32 on args[b] bit for bit; tfb200_track_masks_f32 is this entry with n = 1.  The structs are
+ * passed by value (kernel parameter space).  A NULL args or an invalid args[b] returns what tfb200_track_masks_f32
+ * returns for it, and nothing is launched; images with T == 0 are not written.                                    */
+typedef struct TfbTrackMasksArgs {
+  const float* logits;
+  const int32_t* src;
+  const int32_t* ids;
+  const int32_t* prev_label;
+  int32_t* label;
+  int T, h, w, size_h, size_w, crop_h, crop_w, H, W;
+} TfbTrackMasksArgs;
+
+int tfb200_track_masks_batched_f32(const TfbTrackMasksArgs* args, int n, void* stream);
+
 /* COCO run-length encodings of the masks label == ids[t] of a label map (csrc/mask_rle.cu; what pycocotools
  * mask.encode(np.asfortranarray(label == ids[t]))["counts"] holds, for MOTS20Sequence.write_results,
  * datasets/tracking/mots20_sequence.py:72-91).  label [H][W] int32 row-major (e.g. tfb200_track_masks_f32's output);
@@ -410,6 +426,24 @@ size_t tfb200_mask_rle_workspace_bytes(int H, int W, int T);
 int64_t tfb200_mask_rle_max_bytes(int H, int W, int T);
 int tfb200_mask_rle_i32(const int32_t* label, const int32_t* ids, int H, int W, int T, void* workspace,
                         size_t workspace_bytes, int64_t* header, char* chars, int64_t chars_capacity, void* stream);
+
+/* tfb200_mask_rle_i32 for n label maps (1..16, else TFB200_E_SHAPE) at once: map b is maps[b].label [H][W] with its
+ * own H, W, ids and T.  ONE header [2 + 2 * sum(T)] int64 = {status, total bytes, offset[sum T], length[sum T]} and one
+ * character buffer hold every string, tracks ordered map after map and in ids order within a map; each string is
+ * byte-equal to tfb200_mask_rle_i32's for its map.  Each stage is one launch over all maps (nine launches and four
+ * memsets, whatever n), and tfb200_mask_rle_i32 is this entry with n = 1.  Every map must satisfy the single entry's
+ * limits, sum T <= 2^24, and the boundary lists of all maps share int32 offsets: sum over maps of 2 H W must be
+ * < 2^31, else TFB200_E_SHAPE (and the size queries return 0).  A map with T == 0 has no strings.                 */
+typedef struct TfbMaskRleMap {
+  const int32_t* label;
+  const int32_t* ids;
+  int H, W, T;
+} TfbMaskRleMap;
+
+size_t tfb200_mask_rle_batched_workspace_bytes(const TfbMaskRleMap* maps, int n);
+int64_t tfb200_mask_rle_batched_max_bytes(const TfbMaskRleMap* maps, int n);
+int tfb200_mask_rle_batched_i32(const TfbMaskRleMap* maps, int n, void* workspace, size_t workspace_bytes,
+                                int64_t* header, char* chars, int64_t chars_capacity, void* stream);
 
 /* MOTChallenge CLEAR-MOT and identity metrics of S sequences at once (csrc/mot_eval.cu; what motmetrics 1.2.0
  * computes for get_mot_accum / evaluate_mot_accums, src/trackformer/util/track_utils.py:354-417).  F frames over all

@@ -24,6 +24,11 @@
 //   9. per track: characters written at their offsets (a block scan of the per-count character counts)
 // Buffers are sized for the worst case (every pixel a boundary of two tracks: 2 H W boundaries); a character buffer
 // smaller than the total is reported in the header's status, never truncated.
+//
+// tfb200_mask_rle_batched_i32 runs the same nine launches over up to 16 maps: every stage's grid covers the items
+// (tracks, tiles, chunks) of all maps, and a CTA or warp finds its map in prefix tables passed by value.  Tracks are
+// numbered map after map, so steps 5 and 8 scan all of them at once into one boundary array and one header;
+// tfb200_mask_rle_i32 is the case of one map.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -37,6 +42,7 @@ constexpr int kEventWarps = 4;            // warps (chunks) per block there
 constexpr int kTile = 32;                 // transpose tile
 constexpr int kThreads = 256;             // per-track and scan kernels
 constexpr int kEmpty = -1;                // free hash slot (ids are >= 0)
+constexpr int kMaxBatch = 16;             // maps per call
 
 __device__ __forceinline__ unsigned slot_of(int id, int mask) {
   unsigned x = unsigned(id);
@@ -92,16 +98,49 @@ __device__ __forceinline__ long long block_excl_scan(long long v, long long* war
   return before + inc - v;
 }
 
-// ---- 1. ids -> lowest list position (status bit 1: a negative id)
-__global__ void rle_hash_kernel(const int32_t* __restrict__ ids, int T, int* keys, int* vals, int mask,
+// The maps of one call.  Map b owns the global tracks [t_end[b - 1], t_end[b]), the classify tiles [tile_end[b - 1],
+// tile_end[b]) and the event chunks [chunk_end[b - 1], chunk_end[b]); its hash table, column-major track indices and
+// chunk counts start at hash_off / pix_off / count_off.  A map with T == 0 owns no track, tile or chunk.  Track and chunk indices
+// inside a map are the single-map pipeline's, so each stage runs the single-map body on the map it finds.
+// kCap is the table's capacity: 1 for a single map (the launch then carries a one-entry table and finds its map at
+// compile time), kMaxBatch otherwise.
+template <int kCap>
+struct RleBatch {
+  const int32_t* label[kCap];
+  const int32_t* ids[kCap];
+  int64_t pix_off[kCap];
+  int64_t count_off[kCap];
+  int H[kCap], W[kCap];
+  int t_end[kCap], tile_end[kCap], chunk_end[kCap];
+  int hash_off[kCap], hash_mask[kCap], n_chunks[kCap], tiles_x[kCap];
+};
+
+// the map owning item v of a prefix `end` (v < end[kCap - 1])
+template <int kCap>
+__device__ __forceinline__ int map_of(const int* end, int v) {
+  int b = 0;
+  if (kCap > 1)
+    while (v >= end[b]) ++b;
+  return b;
+}
+
+__device__ __forceinline__ int begin_of(const int* end, int b) { return b ? end[b - 1] : 0; }
+
+// ---- 1. ids -> lowest list position within the map (status bit 1: a negative id)
+template <int kCap>
+__global__ void rle_hash_kernel(const __grid_constant__ RleBatch<kCap> m, int T, int* keys, int* vals,
                                 unsigned long long* status) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= T) return;
-  const int id = ids[t];
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= T) return;
+  const int b = map_of<kCap>(m.t_end, g), t = g - begin_of(m.t_end, b);
+  const int id = m.ids[b][t];
   if (id < 0) {
     atomicOr(status, 1ull);
     return;
   }
+  const int mask = m.hash_mask[b];
+  keys += m.hash_off[b];
+  vals += m.hash_off[b];
   unsigned s = slot_of(id, mask);
   while (true) {
     const int old = atomicCAS(keys + s, kEmpty, id);
@@ -113,12 +152,19 @@ __global__ void rle_hash_kernel(const int32_t* __restrict__ ids, int T, int* key
   }
 }
 
-// ---- 2. row-major label map -> column-major track index (-1: no track)
+// ---- 2. row-major label map -> column-major track index within the map (-1: no track)
+template <int kCap>
 __global__ void __launch_bounds__(kTile * 8)
-rle_classify_kernel(const int32_t* __restrict__ label, const int* __restrict__ keys, const int* __restrict__ vals,
-                    int mask, int* __restrict__ tcm, int H, int W) {
+rle_classify_kernel(const __grid_constant__ RleBatch<kCap> m, const int* __restrict__ keys, const int* __restrict__ vals,
+                    int* __restrict__ tcm) {
   __shared__ int tile[kTile][kTile + 1];
-  const int x0 = blockIdx.x * kTile, y0 = blockIdx.y * kTile;
+  const int b = map_of<kCap>(m.tile_end, blockIdx.x), i = blockIdx.x - begin_of(m.tile_end, b);
+  const int H = m.H[b], W = m.W[b], mask = m.hash_mask[b];
+  const int32_t* __restrict__ label = m.label[b];
+  keys += m.hash_off[b];
+  vals += m.hash_off[b];
+  tcm += m.pix_off[b];
+  const int x0 = (i % m.tiles_x[b]) * kTile, y0 = (i / m.tiles_x[b]) * kTile;
   const int tx = threadIdx.x, ty = threadIdx.y;
 #pragma unroll
   for (int r = 0; r < kTile; r += 8) {
@@ -133,15 +179,20 @@ rle_classify_kernel(const int32_t* __restrict__ label, const int* __restrict__ k
   }
 }
 
-// ---- 3 / 6. boundary events of one chunk per warp.  counts[t * n_chunks + c]: pass 3 counts, pass 6 consumes them as
-// running offsets (after step 4 made them exclusive prefixes) and writes bnd[tbase[t] + offset].
-template <bool kWrite>
+// ---- 3 / 6. boundary events of one chunk per warp.  counts[t * n_chunks + c] of the chunk's map: pass 3 counts, pass
+// 6 consumes them as running offsets (after step 4 made them exclusive prefixes) and writes bnd[tbase[t] + offset].
+template <bool kWrite, int kCap>
 __global__ void __launch_bounds__(32 * kEventWarps)
-rle_events_kernel(const int* __restrict__ tcm, int N, int n_chunks, int* counts, const int* __restrict__ tbase,
-                  int* __restrict__ bnd) {
+rle_events_kernel(const __grid_constant__ RleBatch<kCap> m, int total_chunks, const int* __restrict__ tcm, int* counts,
+                  const int* __restrict__ tbase, int* __restrict__ bnd) {
   const int lane = threadIdx.x & 31;
-  const int c = blockIdx.x * kEventWarps + (threadIdx.x >> 5);
-  if (c >= n_chunks) return;                // whole warps leave together
+  const int cg = blockIdx.x * kEventWarps + (threadIdx.x >> 5);
+  if (cg >= total_chunks) return;           // whole warps leave together
+  const int b = map_of<kCap>(m.chunk_end, cg), c = cg - begin_of(m.chunk_end, b);
+  const int N = m.H[b] * m.W[b], n_chunks = m.n_chunks[b];
+  tcm += m.pix_off[b];
+  counts += m.count_off[b];
+  if (kWrite) tbase += begin_of(m.t_end, b);
   const unsigned lt = (1u << lane) - 1u;
   const int end = min(N, (c + 1) * kChunk);
   for (int p0 = c * kChunk; p0 < end; p0 += 32) {
@@ -157,12 +208,12 @@ rle_events_kernel(const int* __restrict__ tcm, int N, int n_chunks, int* counts,
       const int ka = __shfl_sync(0xffffffffu, prev, src), kb = __shfl_sync(0xffffffffu, cur, src);
       const int X = pa ? ka : kb;
       const bool in_a = need_a && prev == X, in_b = need_b && cur == X;   // at most one: prev != cur
-      const unsigned m = __ballot_sync(0xffffffffu, in_a || in_b);
+      const unsigned msk = __ballot_sync(0xffffffffu, in_a || in_b);
       int* slot = counts + int64_t(X) * n_chunks + c;
       const int before = *slot;
-      if (kWrite && (in_a || in_b)) bnd[tbase[X] + before + __popc(m & lt)] = p;
+      if (kWrite && (in_a || in_b)) bnd[tbase[X] + before + __popc(msk & lt)] = p;
       __syncwarp();
-      if (lane == 0) *slot = before + __popc(m);
+      if (lane == 0) *slot = before + __popc(msk);
       __syncwarp();
       need_a = need_a && !in_a;
       need_b = need_b && !in_b;
@@ -170,13 +221,16 @@ rle_events_kernel(const int* __restrict__ tcm, int N, int n_chunks, int* counts,
   }
 }
 
-// ---- 4. per track: exclusive scan of its chunk counts; also its list's owner (lowest t of the same id)
+// ---- 4. per track: exclusive scan of its chunk counts; also its list's owner (lowest t of the same id in its map)
+template <int kCap>
 __global__ void __launch_bounds__(kThreads)
-rle_track_scan_kernel(const int32_t* __restrict__ ids, const int* __restrict__ keys, const int* __restrict__ vals,
-                      int mask, int* counts, int n_chunks, int* __restrict__ nb, int* __restrict__ rep) {
+rle_track_scan_kernel(const __grid_constant__ RleBatch<kCap> m, const int* __restrict__ keys, const int* __restrict__ vals,
+                      int* counts, int* __restrict__ nb, int* __restrict__ rep) {
   __shared__ long long ws[kThreads / 32];
-  const int t = blockIdx.x;
-  int* row = counts + int64_t(t) * n_chunks;
+  const int g = blockIdx.x;
+  const int b = map_of<kCap>(m.t_end, g), t0 = begin_of(m.t_end, b), t = g - t0;
+  const int n_chunks = m.n_chunks[b];
+  int* row = counts + m.count_off[b] + int64_t(t) * n_chunks;
   long long carry = 0;
   for (int i0 = 0; i0 < n_chunks; i0 += kThreads) {
     const int i = i0 + threadIdx.x;
@@ -187,14 +241,14 @@ rle_track_scan_kernel(const int32_t* __restrict__ ids, const int* __restrict__ k
     carry += total;
   }
   if (threadIdx.x == 0) {
-    nb[t] = int(carry);
-    const int r = lookup(keys, vals, ids[t], mask);
-    rep[t] = r < 0 ? t : r;                 // a negative id has no list (status bit 1 reports it)
+    nb[g] = int(carry);
+    const int r = lookup(keys + m.hash_off[b], vals + m.hash_off[b], m.ids[b][t], m.hash_mask[b]);
+    rep[g] = t0 + (r < 0 ? t : r);          // a negative id has no list (status bit 1 reports it)
   }
 }
 
-// ---- 5 / 8. exclusive scan over tracks (one block).  5: int boundary counts -> list starts.  8: int64 string lengths
-// -> header {status, total, offsets[T], lengths[T]}; status bit 2 when the total exceeds the character buffer.
+// ---- 5 / 8. exclusive scan over all tracks (one block).  5: int boundary counts -> list starts.  8: int64 string
+// lengths -> header {status, total, offsets[T], lengths[T]}; status bit 2 when the total exceeds the character buffer.
 __global__ void __launch_bounds__(kThreads)
 rle_scan_tracks_kernel(const int* __restrict__ nb, int* __restrict__ tbase, const long long* __restrict__ len,
                        long long* __restrict__ header, int T, long long capacity) {
@@ -231,13 +285,15 @@ __device__ __forceinline__ long long count_diff(const int* b, int k, int N, int 
 }
 
 // ---- 7 / 9. per track: 7 sums the characters of its k + 1 counts; 9 writes them at header offsets
-template <bool kWrite>
+template <bool kWrite, int kCap>
 __global__ void __launch_bounds__(kThreads)
-rle_chars_kernel(const int* __restrict__ bnd, const int* __restrict__ tbase, const int* __restrict__ nb,
-                 const int* __restrict__ rep, int N, long long* __restrict__ len, const long long* __restrict__ header,
-                 int T, long long capacity, char* __restrict__ chars) {
+rle_chars_kernel(const __grid_constant__ RleBatch<kCap> m, const int* __restrict__ bnd, const int* __restrict__ tbase,
+                 const int* __restrict__ nb, const int* __restrict__ rep, long long* __restrict__ len,
+                 const long long* __restrict__ header, long long capacity, char* __restrict__ chars) {
   __shared__ long long ws[kThreads / 32];
   const int t = blockIdx.x;
+  const int mb = map_of<kCap>(m.t_end, t);
+  const int N = m.H[mb] * m.W[mb];
   const int r = rep[t];
   const int k = nb[r];
   const int* b = bnd + tbase[r];
@@ -280,50 +336,132 @@ int hash_slots(int T) {
 
 struct Layout {
   size_t keys, vals, rep, nb, tbase, len, counts, tcm, bnd, total;
+  int T, slots, tiles, chunks;
 };
-
-Layout layout(int H, int W, int T) {
-  const size_t N = size_t(H) * W, S = size_t(hash_slots(T)), n_chunks = (N + kChunk - 1) / kChunk;
-  Layout l;
-  size_t o = 0;
-  l.keys = o;   o += align256(S * 4);
-  l.vals = o;   o += align256(S * 4);
-  l.rep = o;    o += align256(size_t(T) * 4);
-  l.nb = o;     o += align256(size_t(T) * 4);
-  l.tbase = o;  o += align256(size_t(T) * 4);
-  l.len = o;    o += align256(size_t(T) * 8);
-  l.counts = o; o += align256(size_t(T) * n_chunks * 4);
-  l.tcm = o;    o += align256(N * 4);
-  l.bnd = o;    o += align256(2 * N * 4);               // each pixel ends at most one run and starts at most one
-  l.total = o;
-  return l;
-}
 
 bool bad_shape(int H, int W, int T) {
   return H <= 0 || W <= 0 || T < 0 || T > (1 << 24) || int64_t(H) * W > (int64_t(1) << 28);
 }
 
-}  // namespace
-
-extern "C" size_t tfb200_mask_rle_workspace_bytes(int H, int W, int T) {
-  return bad_shape(H, W, T) ? 0 : layout(H, W, T).total;
+// Checks the maps (TFB200_E_SHAPE for any bad one, or for sum 2 H W >= 2^31) and lays the workspace out: each region
+// holds the maps' parts back to back, so one map lays out exactly as the single-map pipeline always has.
+int plan(const TfbMaskRleMap* maps, int n, RleBatch<kMaxBatch>* m, Layout* l) {
+  if (n <= 0 || n > kMaxBatch) return TFB200_E_SHAPE;
+  int64_t T = 0, S = 0, N = 0, counts = 0, tiles = 0, chunks = 0, all_pixels = 0;
+  for (int b = 0; b < n; ++b) {
+    const TfbMaskRleMap& a = maps[b];
+    if (bad_shape(a.H, a.W, a.T)) return TFB200_E_SHAPE;
+    all_pixels += int64_t(a.H) * a.W;
+    const bool on = a.T > 0;                // a map without tracks keeps its regions but owns no tiles or chunks
+    const int64_t pixels = int64_t(a.H) * a.W, n_chunks = (pixels + kChunk - 1) / kChunk;
+    const int slots = hash_slots(a.T);
+    m->label[b] = a.label;
+    m->ids[b] = a.ids;
+    m->H[b] = a.H;
+    m->W[b] = a.W;
+    m->hash_off[b] = int(S);
+    m->hash_mask[b] = slots - 1;
+    m->pix_off[b] = N;
+    m->count_off[b] = counts;
+    m->n_chunks[b] = int(n_chunks);
+    m->tiles_x[b] = (a.W + kTile - 1) / kTile;
+    T += a.T;
+    S += slots;
+    N += pixels;
+    counts += int64_t(a.T) * n_chunks;
+    chunks += on ? n_chunks : 0;
+    tiles += on ? int64_t(m->tiles_x[b]) * ((a.H + kTile - 1) / kTile) : 0;
+    m->t_end[b] = int(T);
+    m->chunk_end[b] = int(chunks);
+    m->tile_end[b] = int(tiles);
+  }
+  if (2 * all_pixels >= (int64_t(1) << 31) || T > (1 << 24)) return TFB200_E_SHAPE;
+  for (int b = n; b < kMaxBatch; ++b) {
+    m->t_end[b] = int(T);
+    m->chunk_end[b] = int(chunks);
+    m->tile_end[b] = int(tiles);
+  }
+  size_t o = 0;
+  l->keys = o;   o += align256(size_t(S) * 4);
+  l->vals = o;   o += align256(size_t(S) * 4);
+  l->rep = o;    o += align256(size_t(T) * 4);
+  l->nb = o;     o += align256(size_t(T) * 4);
+  l->tbase = o;  o += align256(size_t(T) * 4);
+  l->len = o;    o += align256(size_t(T) * 8);
+  l->counts = o; o += align256(size_t(counts) * 4);
+  l->tcm = o;    o += align256(size_t(N) * 4);
+  l->bnd = o;    o += align256(2 * size_t(N) * 4);       // each pixel ends at most one run and starts at most one
+  l->total = o;
+  l->T = int(T);
+  l->slots = int(S);
+  l->tiles = int(tiles);
+  l->chunks = int(chunks);
+  return 0;
 }
 
-extern "C" int64_t tfb200_mask_rle_max_bytes(int H, int W, int T) {
-  if (bad_shape(H, W, T)) return 0;
+// characters of all strings of one H x W map with T tracks, at most
+int64_t max_bytes(int H, int W, int T) {
   const int64_t N = int64_t(H) * W;
   int per = 1;                              // characters of any |difference| <= N: 2^(5 per - 1) > N
   while ((int64_t(1) << (5 * per - 1)) <= N) ++per;
   return per * (2 * N + T);                 // at most 2N boundaries over all tracks, k + 1 counts per track
 }
 
-extern "C" int tfb200_mask_rle_i32(const int32_t* label, const int32_t* ids, int H, int W, int T, void* workspace,
-                                   size_t workspace_bytes, int64_t* header, char* chars, int64_t chars_capacity,
-                                   void* stream) {
-  if (!label || !ids || !workspace || !header || !chars) return TFB200_E_NULLPTR;
-  if (bad_shape(H, W, T) || chars_capacity < 0) return TFB200_E_SHAPE;
+// the nine launches of one call (after the four memsets)
+template <int kCap>
+void launch_stages(const RleBatch<kCap>& m, const Layout& l, int T, int* keys, int* vals, int* rep, int* nb,
+                   int* tbase, long long* len, int* counts, int* tcm, int* bnd, long long* hdr, char* chars,
+                   int64_t chars_capacity, cudaStream_t s) {
+  rle_hash_kernel<kCap><<<(T + 255) / 256, 256, 0, s>>>(m, T, keys, vals, reinterpret_cast<unsigned long long*>(hdr));
+  rle_classify_kernel<kCap><<<l.tiles, dim3(kTile, 8), 0, s>>>(m, keys, vals, tcm);
+  const int event_blocks = (l.chunks + kEventWarps - 1) / kEventWarps;
+  rle_events_kernel<false, kCap><<<event_blocks, 32 * kEventWarps, 0, s>>>(m, l.chunks, tcm, counts, nullptr, nullptr);
+  rle_track_scan_kernel<kCap><<<T, kThreads, 0, s>>>(m, keys, vals, counts, nb, rep);
+  rle_scan_tracks_kernel<<<1, kThreads, 0, s>>>(nb, tbase, nullptr, nullptr, T, 0);
+  rle_events_kernel<true, kCap><<<event_blocks, 32 * kEventWarps, 0, s>>>(m, l.chunks, tcm, counts, tbase, bnd);
+  rle_chars_kernel<false, kCap><<<T, kThreads, 0, s>>>(m, bnd, tbase, nb, rep, len, nullptr, 0, nullptr);
+  rle_scan_tracks_kernel<<<1, kThreads, 0, s>>>(nullptr, nullptr, len, hdr, T, chars_capacity);
+  rle_chars_kernel<true, kCap><<<T, kThreads, 0, s>>>(m, bnd, tbase, nb, rep, nullptr, hdr, chars_capacity, chars);
+}
+
+}  // namespace
+
+extern "C" size_t tfb200_mask_rle_batched_workspace_bytes(const TfbMaskRleMap* maps, int n) {
+  RleBatch<kMaxBatch> m;
+  Layout l;
+  return maps && plan(maps, n, &m, &l) == 0 ? l.total : 0;
+}
+
+extern "C" int64_t tfb200_mask_rle_batched_max_bytes(const TfbMaskRleMap* maps, int n) {
+  RleBatch<kMaxBatch> m;
+  Layout l;
+  if (!maps || plan(maps, n, &m, &l) != 0) return 0;
+  int64_t total = 0;
+  for (int b = 0; b < n; ++b) total += maps[b].T > 0 ? max_bytes(maps[b].H, maps[b].W, maps[b].T) : 0;
+  return total;
+}
+
+extern "C" size_t tfb200_mask_rle_workspace_bytes(int H, int W, int T) {
+  const TfbMaskRleMap map = {nullptr, nullptr, H, W, T};
+  return tfb200_mask_rle_batched_workspace_bytes(&map, 1);
+}
+
+extern "C" int64_t tfb200_mask_rle_max_bytes(int H, int W, int T) {
+  return bad_shape(H, W, T) ? 0 : max_bytes(H, W, T);
+}
+
+extern "C" int tfb200_mask_rle_batched_i32(const TfbMaskRleMap* maps, int n, void* workspace, size_t workspace_bytes,
+                                           int64_t* header, char* chars, int64_t chars_capacity, void* stream) {
+  if (!maps || !workspace || !header || !chars) return TFB200_E_NULLPTR;
+  if (n <= 0 || n > kMaxBatch) return TFB200_E_SHAPE;
+  for (int b = 0; b < n; ++b)
+    if (!maps[b].label || !maps[b].ids) return TFB200_E_NULLPTR;
+  RleBatch<kMaxBatch> m;
+  Layout l;
+  if (const int rc = plan(maps, n, &m, &l)) return rc;
+  if (chars_capacity < 0) return TFB200_E_SHAPE;
+  const int T = l.T;
   if (T == 0) return 0;
-  const Layout l = layout(H, W, T);
   if (workspace_bytes < l.total) return TFB200_E_SHAPE;
   const cudaStream_t s = cudaStream_t(stream);
   char* ws = static_cast<char*>(workspace);
@@ -337,25 +475,38 @@ extern "C" int tfb200_mask_rle_i32(const int32_t* label, const int32_t* ids, int
   int* tcm = reinterpret_cast<int*>(ws + l.tcm);
   int* bnd = reinterpret_cast<int*>(ws + l.bnd);
   long long* hdr = reinterpret_cast<long long*>(header);
-  const int N = H * W, S = hash_slots(T), n_chunks = (N + kChunk - 1) / kChunk;
 
   cudaError_t e;
-  if ((e = cudaMemsetAsync(keys, 0xff, size_t(S) * 4, s)) != cudaSuccess) return int(e);     // kEmpty
-  if ((e = cudaMemsetAsync(vals, 0x7f, size_t(S) * 4, s)) != cudaSuccess) return int(e);     // > any t (atomicMin)
-  if ((e = cudaMemsetAsync(counts, 0, size_t(T) * n_chunks * 4, s)) != cudaSuccess) return int(e);
+  if ((e = cudaMemsetAsync(keys, 0xff, size_t(l.slots) * 4, s)) != cudaSuccess) return int(e);   // kEmpty
+  if ((e = cudaMemsetAsync(vals, 0x7f, size_t(l.slots) * 4, s)) != cudaSuccess) return int(e);   // > any t (atomicMin)
+  if ((e = cudaMemsetAsync(counts, 0, l.tcm - l.counts, s)) != cudaSuccess) return int(e);
   if ((e = cudaMemsetAsync(hdr, 0, sizeof(long long), s)) != cudaSuccess) return int(e);
-  rle_hash_kernel<<<(T + 255) / 256, 256, 0, s>>>(ids, T, keys, vals, S - 1,
-                                                 reinterpret_cast<unsigned long long*>(hdr));
-  rle_classify_kernel<<<dim3((W + kTile - 1) / kTile, (H + kTile - 1) / kTile), dim3(kTile, 8), 0, s>>>(
-      label, keys, vals, S - 1, tcm, H, W);
-  const int event_blocks = (n_chunks + kEventWarps - 1) / kEventWarps;
-  rle_events_kernel<false><<<event_blocks, 32 * kEventWarps, 0, s>>>(tcm, N, n_chunks, counts, nullptr, nullptr);
-  rle_track_scan_kernel<<<T, kThreads, 0, s>>>(ids, keys, vals, S - 1, counts, n_chunks, nb, rep);
-  rle_scan_tracks_kernel<<<1, kThreads, 0, s>>>(nb, tbase, nullptr, nullptr, T, 0);
-  rle_events_kernel<true><<<event_blocks, 32 * kEventWarps, 0, s>>>(tcm, N, n_chunks, counts, tbase, bnd);
-  rle_chars_kernel<false><<<T, kThreads, 0, s>>>(bnd, tbase, nb, rep, N, len, nullptr, T, 0, nullptr);
-  rle_scan_tracks_kernel<<<1, kThreads, 0, s>>>(nullptr, nullptr, len, hdr, T, chars_capacity);
-  rle_chars_kernel<true><<<T, kThreads, 0, s>>>(bnd, tbase, nb, rep, N, nullptr, hdr, T, chars_capacity, chars);
+  if (n == 1) {
+    RleBatch<1> one;
+    one.label[0] = m.label[0];
+    one.ids[0] = m.ids[0];
+    one.pix_off[0] = m.pix_off[0];
+    one.count_off[0] = m.count_off[0];
+    one.H[0] = m.H[0];
+    one.W[0] = m.W[0];
+    one.t_end[0] = m.t_end[0];
+    one.tile_end[0] = m.tile_end[0];
+    one.chunk_end[0] = m.chunk_end[0];
+    one.hash_off[0] = m.hash_off[0];
+    one.hash_mask[0] = m.hash_mask[0];
+    one.n_chunks[0] = m.n_chunks[0];
+    one.tiles_x[0] = m.tiles_x[0];
+    launch_stages(one, l, T, keys, vals, rep, nb, tbase, len, counts, tcm, bnd, hdr, chars, chars_capacity, s);
+  } else {
+    launch_stages(m, l, T, keys, vals, rep, nb, tbase, len, counts, tcm, bnd, hdr, chars, chars_capacity, s);
+  }
   msda_b200_count_launches(9);
   return int(cudaGetLastError());
+}
+
+extern "C" int tfb200_mask_rle_i32(const int32_t* label, const int32_t* ids, int H, int W, int T, void* workspace,
+                                   size_t workspace_bytes, int64_t* header, char* chars, int64_t chars_capacity,
+                                   void* stream) {
+  const TfbMaskRleMap map = {label, ids, H, W, T};
+  return tfb200_mask_rle_batched_i32(&map, 1, workspace, workspace_bytes, header, chars, chars_capacity, stream);
 }

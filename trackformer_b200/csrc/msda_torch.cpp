@@ -17,6 +17,7 @@
 #include <c10/cuda/CUDAStream.h>
 
 #include <algorithm>
+#include <map>
 #include <vector>
 
 #include "../../include/msda_b200.h"
@@ -1426,73 +1427,126 @@ at::Tensor mask_loss_backward(const at::Tensor& logits, const at::Tensor& src, c
 }
 
 // ---- tracker segmentation masks (csrc/track_masks.cu) ----
+// Image b: logits [K, h, w] fp32, src / ids [T] int32, prev_label [H, W] int32 or None, geom {size_h, size_w, crop_h,
+// crop_w, H, W} -> label [H, W] int32.  One launch for all images (images with T == 0 stay all background).
+std::vector<at::Tensor> track_masks_batched(const std::vector<at::Tensor>& logits, const std::vector<at::Tensor>& src,
+                                            const std::vector<at::Tensor>& ids,
+                                            const std::vector<c10::optional<at::Tensor>>& prev_label,
+                                            const std::vector<std::vector<int64_t>>& geom) {
+  const size_t n = logits.size();
+  TORCH_CHECK(n >= 1 && n <= 16, "track_masks: 1 to 16 images per call, got ", n);
+  TORCH_CHECK(src.size() == n && ids.size() == n && prev_label.size() == n && geom.size() == n,
+              "track_masks: one src, ids, prev_label and geometry per image");
+  const c10::cuda::CUDAGuard guard(logits[0].device());
+  std::vector<at::Tensor> keep, labels;
+  std::vector<TfbTrackMasksArgs> args(n);
+  for (size_t b = 0; b < n; ++b) {
+    check_f32(logits[b], "track_masks logits");
+    TORCH_CHECK(logits[b].dim() == 3, "track_masks: logits must be [K, h, w]");
+    TORCH_CHECK(logits[b].device() == logits[0].device(), "track_masks: all images on one device");
+    auto check_i32 = [&](const at::Tensor& t, const char* what) {
+      TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kInt && t.device() == logits[b].device(), what,
+                  ": int32 CUDA tensor on the logits' device required");
+    };
+    check_i32(src[b], "track_masks src");
+    check_i32(ids[b], "track_masks ids");
+    TORCH_CHECK(src[b].dim() == 1 && src[b].sizes() == ids[b].sizes(), "track_masks: src and ids must be [T]");
+    TORCH_CHECK(geom[b].size() == 6, "track_masks: geometry is {size_h, size_w, crop_h, crop_w, H, W}");
+    const int64_t H = geom[b][4], W = geom[b][5];
+    const at::Tensor lc = logits[b].contiguous(), sc = src[b].contiguous(), ic = ids[b].contiguous();
+    at::Tensor pc;
+    if (prev_label[b].has_value() && prev_label[b]->defined()) {
+      check_i32(*prev_label[b], "track_masks prev_label");
+      TORCH_CHECK(prev_label[b]->dim() == 2 && prev_label[b]->size(0) == H && prev_label[b]->size(1) == W,
+                  "track_masks: prev_label must be [H, W]");
+      pc = prev_label[b]->contiguous();
+    }
+    labels.push_back(at::full({H, W}, -1, ids[b].options()));
+    const int T = int(src[b].numel());
+    // no active track: all background (empty tensors have no data, and the entry writes nothing for T == 0)
+    args[b] = {lc.numel() ? lc.data_ptr<float>() : nullptr, T ? sc.data_ptr<int32_t>() : nullptr,
+               T ? ic.data_ptr<int32_t>() : nullptr, pc.defined() ? pc.data_ptr<int32_t>() : nullptr,
+               labels.back().data_ptr<int32_t>(), T, int(logits[b].size(1)), int(logits[b].size(2)),
+               int(geom[b][0]), int(geom[b][1]), int(geom[b][2]), int(geom[b][3]), int(H), int(W)};
+    if (T == 0) args[b].src = args[b].ids = labels.back().data_ptr<int32_t>();   // non-NULL, never read
+    keep.insert(keep.end(), {lc, sc, ic, pc});
+  }
+  raise_rc(tfb200_track_masks_batched_f32(args.data(), int(n), c10::cuda::getCurrentCUDAStream().stream()),
+           "track_masks");
+  return labels;
+}
+
 // logits [K, h, w] fp32, src / ids [T] int32, prev_label [H, W] int32 or None -> label [H, W] int32
 at::Tensor track_masks(const at::Tensor& logits, const at::Tensor& src, const at::Tensor& ids,
                        const c10::optional<at::Tensor>& prev_label, int64_t size_h, int64_t size_w, int64_t crop_h,
                        int64_t crop_w, int64_t H, int64_t W) {
-  check_f32(logits, "track_masks logits");
-  TORCH_CHECK(logits.dim() == 3, "track_masks: logits must be [K, h, w]");
-  auto check_i32 = [&](const at::Tensor& t, const char* what) {
-    TORCH_CHECK(t.is_cuda() && t.scalar_type() == at::kInt && t.device() == logits.device(), what,
-                ": int32 CUDA tensor on the logits' device required");
-  };
-  check_i32(src, "track_masks src");
-  check_i32(ids, "track_masks ids");
-  TORCH_CHECK(src.dim() == 1 && src.sizes() == ids.sizes(), "track_masks: src and ids must be [T]");
-  const at::Tensor lc = logits.contiguous(), sc = src.contiguous(), ic = ids.contiguous();
-  at::Tensor pc;
-  if (prev_label.has_value() && prev_label->defined()) {
-    check_i32(*prev_label, "track_masks prev_label");
-    TORCH_CHECK(prev_label->dim() == 2 && prev_label->size(0) == H && prev_label->size(1) == W,
-                "track_masks: prev_label must be [H, W]");
-    pc = prev_label->contiguous();
-  }
-  const c10::cuda::CUDAGuard guard(logits.device());
-  at::Tensor label = at::full({H, W}, -1, ids.options());
-  if (src.numel() == 0) return label;                  // no active track: all background (empty tensors have no data)
-  raise_rc(tfb200_track_masks_f32(lc.numel() ? lc.data_ptr<float>() : nullptr, sc.data_ptr<int32_t>(),
-                                  ic.data_ptr<int32_t>(), pc.defined() ? pc.data_ptr<int32_t>() : nullptr,
-                                  label.data_ptr<int32_t>(), int(src.numel()), int(logits.size(1)),
-                                  int(logits.size(2)), int(size_h), int(size_w), int(crop_h), int(crop_w), int(H),
-                                  int(W), c10::cuda::getCurrentCUDAStream().stream()),
-           "track_masks");
-  return label;
+  return track_masks_batched({logits}, {src}, {ids}, {prev_label}, {{size_h, size_w, crop_h, crop_w, H, W}})[0];
 }
 
-// ---- COCO RLE strings of a label map's per-track masks (csrc/mask_rle.cu) ----
-// label [H, W] int32, ids [T] int32 on one device -> T bytes objects.  Two device-to-host copies: the header (offsets,
-// lengths) and then exactly the string bytes; the label map stays on the device.
-std::vector<pybind11::bytes> mask_rle(const at::Tensor& label, const at::Tensor& ids) {
-  TORCH_CHECK(label.is_cuda() && label.scalar_type() == at::kInt && label.dim() == 2,
-              "mask_rle label: int32 CUDA tensor [H, W] required");
-  TORCH_CHECK(ids.is_cuda() && ids.scalar_type() == at::kInt && ids.dim() == 1 && ids.device() == label.device(),
-              "mask_rle ids: int32 CUDA tensor [T] on the label map's device required");
-  const int64_t H = label.size(0), W = label.size(1), T = ids.size(0);
-  TORCH_CHECK(H > 0 && W > 0 && H * W <= (int64_t(1) << 28) && T <= (int64_t(1) << 24),
-              "mask_rle: H, W > 0, H * W <= 2^28 and T <= 2^24 required");
-  if (T == 0) return {};
-  const c10::cuda::CUDAGuard guard(label.device());
-  const at::Tensor lc = label.contiguous(), ic = ids.contiguous();
-  const auto u8 = lc.options().dtype(at::kByte);
-  const size_t ws_bytes = tfb200_mask_rle_workspace_bytes(int(H), int(W), int(T));
-  const int64_t cap = tfb200_mask_rle_max_bytes(int(H), int(W), int(T));
-  at::Tensor ws = at::empty({int64_t(ws_bytes)}, u8);
-  at::Tensor chars = at::empty({cap}, u8);
-  at::Tensor header = at::empty({2 + 2 * T}, lc.options().dtype(at::kLong));
-  raise_rc(tfb200_mask_rle_i32(lc.data_ptr<int32_t>(), ic.data_ptr<int32_t>(), int(H), int(W), int(T), ws.data_ptr(),
-                               ws_bytes, header.data_ptr<int64_t>(), reinterpret_cast<char*>(chars.data_ptr()), cap,
-                               c10::cuda::getCurrentCUDAStream().stream()),
+// ---- COCO RLE strings of label maps' per-track masks (csrc/mask_rle.cu) ----
+// labels[b] [H_b, W_b] int32, ids[b] [T_b] int32, all on one device -> per map T_b bytes objects.  One call of the
+// batched entry and two device-to-host copies whatever the number of maps: the header (offsets, lengths) and then
+// exactly the string bytes; the label maps stay on the device.  The workspace, header and character buffers persist
+// per device and grow on demand (the worst case of a 1080 x 1920 map is ~25 MB of workspace and ~21 MB of characters).
+std::vector<std::vector<pybind11::bytes>> mask_rle_batched(const std::vector<at::Tensor>& labels,
+                                                           const std::vector<at::Tensor>& ids) {
+  const size_t n = labels.size();
+  TORCH_CHECK(n >= 1 && n <= 16, "mask_rle: 1 to 16 label maps per call, got ", n);
+  TORCH_CHECK(ids.size() == n, "mask_rle: one ids tensor per label map");
+  std::vector<at::Tensor> keep;
+  std::vector<TfbMaskRleMap> maps(n);
+  int64_t T = 0;
+  for (size_t b = 0; b < n; ++b) {
+    const at::Tensor& label = labels[b];
+    TORCH_CHECK(label.is_cuda() && label.scalar_type() == at::kInt && label.dim() == 2 &&
+                label.device() == labels[0].device(), "mask_rle label: int32 CUDA tensor [H, W] required");
+    TORCH_CHECK(ids[b].is_cuda() && ids[b].scalar_type() == at::kInt && ids[b].dim() == 1 &&
+                ids[b].device() == label.device(), "mask_rle ids: int32 CUDA tensor [T] on the label map's device required");
+    const int64_t H = label.size(0), W = label.size(1), Tb = ids[b].size(0);
+    TORCH_CHECK(H > 0 && W > 0 && H * W <= (int64_t(1) << 28) && Tb <= (int64_t(1) << 24),
+                "mask_rle: H, W > 0, H * W <= 2^28 and T <= 2^24 required");
+    const at::Tensor lc = label.contiguous(), ic = ids[b].contiguous();
+    maps[b] = {lc.data_ptr<int32_t>(), Tb ? ic.data_ptr<int32_t>() : lc.data_ptr<int32_t>(), int(H), int(W), int(Tb)};
+    keep.insert(keep.end(), {lc, ic});
+    T += Tb;
+  }
+  std::vector<std::vector<pybind11::bytes>> out(n);
+  if (T == 0) return out;
+  const size_t ws_bytes = tfb200_mask_rle_batched_workspace_bytes(maps.data(), int(n));
+  const int64_t cap = tfb200_mask_rle_batched_max_bytes(maps.data(), int(n));
+  TORCH_CHECK(ws_bytes > 0, "mask_rle: the maps' boundary lists exceed 2^31 entries (sum of 2 H W)");
+  const c10::cuda::CUDAGuard guard(labels[0].device());
+  struct Buffers {
+    at::Tensor ws, chars, header;
+  };
+  static auto* cache = new std::map<int, Buffers>();      // never destroyed: no CUDA frees at interpreter exit
+  Buffers& buf = (*cache)[labels[0].get_device()];
+  const auto u8 = labels[0].options().dtype(at::kByte);
+  if (!buf.ws.defined() || buf.ws.numel() < int64_t(ws_bytes)) buf.ws = at::empty({int64_t(ws_bytes)}, u8);
+  if (!buf.chars.defined() || buf.chars.numel() < cap) buf.chars = at::empty({cap}, u8);
+  if (!buf.header.defined() || buf.header.numel() < 2 + 2 * T)
+    buf.header = at::empty({2 + 2 * T}, labels[0].options().dtype(at::kLong));
+  raise_rc(tfb200_mask_rle_batched_i32(maps.data(), int(n), buf.ws.data_ptr(), size_t(buf.ws.numel()),
+                                       buf.header.data_ptr<int64_t>(), reinterpret_cast<char*>(buf.chars.data_ptr()),
+                                       cap, c10::cuda::getCurrentCUDAStream().stream()),
            "mask_rle");
-  const at::Tensor h = header.cpu();
+  const at::Tensor h = buf.header.narrow(0, 0, 2 + 2 * T).cpu();
   const int64_t* hp = h.data_ptr<int64_t>();
   TORCH_CHECK(!(hp[0] & 1), "mask_rle: ids must be >= 0");
   TORCH_CHECK(hp[0] == 0, "mask_rle: ", hp[1], " string bytes exceed the bound of ", cap);
-  const at::Tensor s = chars.narrow(0, 0, hp[1]).cpu();
+  const at::Tensor s = buf.chars.narrow(0, 0, hp[1]).cpu();
   const char* sp = reinterpret_cast<const char*>(s.data_ptr());
-  std::vector<pybind11::bytes> out;
-  out.reserve(size_t(T));
-  for (int64_t t = 0; t < T; ++t) out.emplace_back(sp + hp[2 + t], size_t(hp[2 + T + t]));
+  int64_t g = 0;
+  for (size_t b = 0; b < n; ++b) {
+    out[b].reserve(size_t(maps[b].T));
+    for (int t = 0; t < maps[b].T; ++t, ++g) out[b].emplace_back(sp + hp[2 + g], size_t(hp[2 + T + g]));
+  }
   return out;
+}
+
+// label [H, W] int32, ids [T] int32 on one device -> T bytes objects (mask_rle_batched of one map)
+std::vector<pybind11::bytes> mask_rle(const at::Tensor& label, const at::Tensor& ids) {
+  return mask_rle_batched({label}, {ids})[0];
 }
 
 // ---- frame ingest (csrc/frame_ingest.cu) ----
@@ -1602,6 +1656,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("mask_loss_forward", &mask_loss_forward);
   m.def("mask_loss_backward", &mask_loss_backward);
   m.def("track_masks", &track_masks);
+  m.def("track_masks_batched", &track_masks_batched);
   m.def("mask_rle", &mask_rle);
+  m.def("mask_rle_batched", &mask_rle_batched);
   m.def("frame_ingest", &frame_ingest);
 }

@@ -35,6 +35,7 @@ constexpr int kRows = kTileH / (kThreads / kTileW);
 constexpr int kMaxChunk = 256;             // tracks per pass over the output tile
 constexpr int kStageFloats = 8192;         // 32 KB of staged logits per pass
 constexpr int kMaxSmem = 200 * 1024;
+constexpr int kMaxBatch = 16;             // images per launch
 
 struct Lin {
   int i0, i1;
@@ -67,10 +68,35 @@ __device__ __forceinline__ unsigned slot_of(int id, int mask) {
   return (x ^ (x >> 16)) & unsigned(mask);
 }
 
+// The images of one launch.  Image b owns the output tiles [tile_end[b - 1], tile_end[b]) of the 1-D grid; every CTA
+// works on one tile of one image, so the body below is the single-image kernel with that image's arguments.
+// tfb200_track_masks_f32 is the launch of one image.
+// kCap is the table's capacity: 1 for a single image (a one-entry table, the image known at compile time), else
+// kMaxBatch.
+template <int kCap>
+struct MasksBatch {
+  TfbTrackMasksArgs a[kCap];
+  int tiles_x[kCap];
+  int tile_end[kCap];
+  int hash_slots;                          // the largest stale set's table; a larger table maps ids to the same t
+};
+
+template <int kCap>
 __global__ void __launch_bounds__(kThreads, 2)
-track_masks_kernel(const float* __restrict__ logits, const int32_t* __restrict__ src, const int32_t* __restrict__ ids,
-                   const int32_t* __restrict__ prev, int32_t* __restrict__ label, int T, int h, int w, int size_h,
-                   int size_w, int crop_h, int crop_w, int H, int W, int hash_slots) {
+track_masks_kernel(const __grid_constant__ MasksBatch<kCap> batch) {
+  int b = 0;
+  if (kCap > 1)
+    while (int(blockIdx.x) >= batch.tile_end[b]) ++b;
+  const TfbTrackMasksArgs& a = batch.a[b];
+  const float* __restrict__ logits = a.logits;
+  const int32_t* __restrict__ src = a.src;
+  const int32_t* __restrict__ ids = a.ids;
+  const int32_t* __restrict__ prev = a.prev_label;
+  int32_t* __restrict__ label = a.label;
+  const int T = a.T, h = a.h, w = a.w, size_h = a.size_h, size_w = a.size_w, crop_h = a.crop_h, crop_w = a.crop_w;
+  const int H = a.H, W = a.W, hash_slots = batch.hash_slots;
+  const int tile = int(blockIdx.x) - (b ? batch.tile_end[b - 1] : 0);
+  const int tile_x = tile % batch.tiles_x[b], tile_y = tile / batch.tiles_x[b];
   extern __shared__ int smem[];
   int* hkey = smem;
   int* hval = hkey + hash_slots;
@@ -95,7 +121,7 @@ track_masks_kernel(const float* __restrict__ logits, const int32_t* __restrict__
   }
 
   // ---- source indices of this thread's pixels, and the tile's low-resolution footprint (indices are monotone)
-  const int x0_tile = blockIdx.x * kTileW, y0_tile = blockIdx.y * kTileH;
+  const int x0_tile = tile_x * kTileW, y0_tile = tile_y * kTileH;
   const int x_last = min(x0_tile + kTileW, W) - 1, y_last = min(y0_tile + kTileH, H) - 1;
   const int fx0 = linear_src(nearest_src(x0_tile, crop_w, W), w, size_w).i0;
   const int fx1 = linear_src(nearest_src(x_last, crop_w, W), w, size_w).i1;
@@ -183,26 +209,66 @@ int next_pow2(int v) {
   return p;
 }
 
+template <int kCap>
+cudaError_t launch(const MasksBatch<kCap>& batch, int tiles, size_t smem, cudaStream_t s) {
+  if (smem > 48 * 1024) {
+    const cudaError_t e =
+        cudaFuncSetAttribute(track_masks_kernel<kCap>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
+    if (e != cudaSuccess) return e;
+  }
+  track_masks_kernel<kCap><<<tiles, kThreads, smem, s>>>(batch);
+  return cudaSuccess;
+}
+
+bool bad_args(const TfbTrackMasksArgs& a) {
+  return a.T < 0 || a.h <= 0 || a.w <= 0 || a.size_h <= 0 || a.size_w <= 0 || a.crop_h <= 0 || a.crop_w <= 0 ||
+         a.crop_h > a.size_h || a.crop_w > a.size_w || a.H <= 0 || a.W <= 0 || a.T > (1 << 24);
+}
+
 }  // namespace
+
+extern "C" int tfb200_track_masks_batched_f32(const TfbTrackMasksArgs* args, int n, void* stream) {
+  if (!args) return TFB200_E_NULLPTR;
+  if (n <= 0 || n > kMaxBatch) return TFB200_E_SHAPE;
+  MasksBatch<kMaxBatch> batch;
+  int tiles = 0, max_stale = 0;
+  for (int b = 0; b < n; ++b) {
+    const TfbTrackMasksArgs& a = args[b];
+    if (!a.src || !a.ids || !a.label) return TFB200_E_NULLPTR;
+    if (bad_args(a)) return TFB200_E_SHAPE;
+    batch.a[b] = a;
+    batch.tiles_x[b] = (a.W + kTileW - 1) / kTileW;
+    const int64_t own = a.T == 0 ? 0 : int64_t(batch.tiles_x[b]) * ((a.H + kTileH - 1) / kTileH);   // T == 0: untouched
+    if (tiles + own > int64_t(INT32_MAX)) return TFB200_E_SHAPE;
+    tiles += int(own);
+    batch.tile_end[b] = tiles;
+    if (a.T > 0 && a.prev_label) max_stale = a.T > max_stale ? a.T : max_stale;
+  }
+  for (int b = n; b < kMaxBatch; ++b) batch.tile_end[b] = tiles;
+  if (tiles == 0) return 0;
+  batch.hash_slots = max_stale ? next_pow2(2 * max_stale) : 0;
+  const size_t smem = (size_t(2) * batch.hash_slots + kMaxChunk) * sizeof(int) + kStageFloats * sizeof(float);
+  if (smem > size_t(kMaxSmem)) return TFB200_E_SHAPE;
+  const cudaStream_t s = cudaStream_t(stream);
+  cudaError_t e;
+  if (n == 1) {
+    MasksBatch<1> one;
+    one.a[0] = batch.a[0];
+    one.tiles_x[0] = batch.tiles_x[0];
+    one.tile_end[0] = batch.tile_end[0];
+    one.hash_slots = batch.hash_slots;
+    e = launch(one, tiles, smem, s);
+  } else {
+    e = launch(batch, tiles, smem, s);
+  }
+  if (e != cudaSuccess) return int(e);
+  msda_b200_count_launches(1);
+  return int(cudaGetLastError());
+}
 
 extern "C" int tfb200_track_masks_f32(const float* logits, const int32_t* src, const int32_t* ids,
                                       const int32_t* prev_label, int32_t* label, int T, int h, int w, int size_h,
                                       int size_w, int crop_h, int crop_w, int H, int W, void* stream) {
-  if (!src || !ids || !label) return TFB200_E_NULLPTR;
-  if (T < 0 || h <= 0 || w <= 0 || size_h <= 0 || size_w <= 0 || crop_h <= 0 || crop_w <= 0 || crop_h > size_h ||
-      crop_w > size_w || H <= 0 || W <= 0 || T > (1 << 24))
-    return TFB200_E_SHAPE;
-  if (T == 0) return 0;
-  const int hash_slots = prev_label ? next_pow2(2 * T) : 0;
-  const size_t smem = (size_t(2) * hash_slots + kMaxChunk) * sizeof(int) + kStageFloats * sizeof(float);
-  if (smem > size_t(kMaxSmem)) return TFB200_E_SHAPE;
-  if (smem > 48 * 1024) {
-    const cudaError_t e = cudaFuncSetAttribute(track_masks_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem));
-    if (e != cudaSuccess) return int(e);
-  }
-  const dim3 grid((W + kTileW - 1) / kTileW, (H + kTileH - 1) / kTileH);
-  track_masks_kernel<<<grid, kThreads, smem, cudaStream_t(stream)>>>(logits, src, ids, prev_label, label, T, h, w, size_h,
-                                                                     size_w, crop_h, crop_w, H, W, hash_slots);
-  msda_b200_count_launches(1);
-  return int(cudaGetLastError());
+  const TfbTrackMasksArgs a = {logits, src, ids, prev_label, label, T, h, w, size_h, size_w, crop_h, crop_w, H, W};
+  return tfb200_track_masks_batched_f32(&a, 1, stream);
 }

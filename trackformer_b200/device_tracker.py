@@ -239,18 +239,27 @@ class DeviceTracker(Tracker):
         a.detection_nms_on, a.track_nms_on = int(bool(self.detection_nms_thresh)), int(bool(self.track_nms_thresh))
         return a
 
-    def _take_results(self, out, det_out, blob, height, width):
-        """Book the frame from its read-back words `out` (header + result rows) and advance to the next frame."""
-        n_active, n_inactive, track_num, num_reids, n_next, error, n_results = (int(v) for v in out[:7])
+    @staticmethod
+    def _result_body(out):
+        """The result rows [n, 8] int32 of a frame's read-back words `out` (header + result rows): word 0 the track id,
+        word 7 the query row the track took this frame (-1: none).  Raises on an error the kernel reported."""
+        error, n_results = int(out[5]), int(out[6])
         if error:
             raise RuntimeError(f"track_step kernel reported error {error} (1: query count / state mismatch, 2: capacity)")
-        body = out[8:8 + 8 * n_results].reshape(n_results, 8)
+        return out[8:8 + 8 * n_results].reshape(n_results, 8)
+
+    def _take_results(self, out, det_out, blob, height, width, masks=None, maps=None):
+        """Book the frame from its read-back words `out` (header + result rows) and advance to the next frame.  The
+        results' `masks` / attention `maps` (in result order) are made here from `det_out` unless the caller hands
+        them in (MultiSequenceTracker makes them for all its sequences at once)."""
+        body = self._result_body(out)
+        n_active, n_inactive, track_num, num_reids, n_next = (int(v) for v in out[:5])
+        n_results = len(body)
         fbody = body.view(np.float32)
         self._result_rows = body[:, 7].astype(np.int64)
-        masks = maps = None
-        if self.masks:
+        if self.masks and masks is None:
             masks = self._resolve_masks(det_out, self._result_rows, body[:, 0], blob, (height, width))
-        if self.generate_attention_maps:
+        if self.generate_attention_maps and maps is None:
             maps = self._attention_maps(det_out, self._result_rows, body[:, 0])
         for k in range(n_results):
             entry = {"bbox": fbody[k, 3:7].copy(), "score": np.array(fbody[k, 2]), "obj_ind": int(body[k, 1])}

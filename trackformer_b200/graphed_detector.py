@@ -21,7 +21,9 @@ the tracker asks for, from the static buffers of the last call.
 `use_graphs=False` keeps the padding but runs the model eagerly (used by the CPU tests of the padding logic).
 
 With the vanilla model's `generate_attention_maps` switch on, the switch is part of the plan key: the captured graph
-computes the maps as one more static output, and `out["attention_maps"]` drops the filler rows like the other outputs.
+computes the maps as one more static output, and `out["attention_maps"]` drops the filler rows like the other outputs
+(`batched` returns them padded, like its other outputs).  `batched_mask_logits` is `mask_logits` for a `batched` call:
+the ragged mask head over a different set of rows per image.
 """
 import torch
 
@@ -50,6 +52,7 @@ class GraphedDetector:
         self.has_mask_head = callable(getattr(model, "mask_logits", None))
         self._plans = {}
         self._last = None
+        self.last_batched = None                     # (plan, K_b) of the last `batched` call, for batched_mask_logits
         self.replays = 0
         self.captures = 0
 
@@ -239,9 +242,11 @@ class GraphedDetector:
         forward = self.model.detect if self.has_mask_head else self.model
         prev_valid = None if plan.prev is None else plan.prev_valid
         with torch.no_grad():
-            out, _, features, _, _ = forward(plan.img, targets, plan.prev, prev_valid)
-        plan.features = features[-3:]
+            out, _, features, plan.memory, plan.hs_all = forward(plan.img, targets, plan.prev, prev_valid)
+        plan.features = features[-3:]                    # what a later call takes as prev_features
+        plan.all_features = features                     # the mask head also reads the stride-4 level
         plan.logits, plan.out_boxes, plan.hs_embed = out["pred_logits"], out["pred_boxes"], out["hs_embed"]
+        plan.attention_maps = out.get("attention_maps")
 
     def batched(self, samples, targets=None, prev_features=None):
         """One forward of B images that each carry their own track queries -- B independent sequences stepped together.
@@ -258,8 +263,10 @@ class GraphedDetector:
         dtype, kb, previous-frame features yes/no); which images have a previous frame is a static input of it.
 
         Returns ``(out, features, ks, kb)``: ``out`` with the padded ``pred_logits`` / ``pred_boxes`` / ``hs_embed``
-        [B, kb + nq, .] (views of the graph's buffers: valid until the next call), the levels ``features`` a later
-        call takes as ``prev_features`` (its own copy), and the host ints K_b."""
+        [B, kb + nq, .] -- and ``attention_maps`` [B, kb + nq, h, w] with the vanilla model's switch on -- (views of
+        the graph's buffers: valid until the next call), the levels ``features`` a later call takes as
+        ``prev_features`` (its own copy), and the host ints K_b.  ``last_batched`` then names this call for
+        ``batched_mask_logits``."""
         if not torch.is_tensor(samples) or samples.ndim != 4:
             raise ValueError("GraphedDetector.batched takes one [B, 3, H, W] tensor of same-sized images")
         bsz = samples.shape[0]
@@ -302,11 +309,40 @@ class GraphedDetector:
             self.replays += 1
         else:
             self._run_batched(plan)
+        self.last_batched = (plan, ks)
         features = plan.features
         if self.uses_prev and plan.graph is not None:
             features = [NestedTensor(f.tensors.clone(), f.mask) for f in plan.features]
         out = {"pred_logits": plan.logits, "pred_boxes": plan.out_boxes, "hs_embed": plan.hs_embed}
+        if plan.attention_maps is not None:
+            out["attention_maps"] = plan.attention_maps
         return out, features, ks, kb
+
+    def batched_mask_logits(self, src_rows, sizes, call=None):
+        """Mask logits ``[sum(sizes), H/4, W/4]`` of rows of a ``batched`` call, computed eagerly by the ragged mask
+        head from that call's static feature / memory / decoder buffers (valid until the next call with the same
+        plan key).  Image b contributes ``sizes[b]`` rows; ``src_rows`` holds them image after image as REAL row
+        indices of the image (``[track queries (K_b) | object queries]``, what the decision kernel reports), which
+        sit at padded row ``kb - K_b + r``.  ``call`` is the ``last_batched`` value right after that call (default:
+        the last call).  Images may contribute no rows."""
+        if not self.has_mask_head:
+            raise RuntimeError("GraphedDetector.batched_mask_logits: the wrapped model has no mask head")
+        if call is None:
+            call = getattr(self, "last_batched", None)
+            if call is None:
+                raise RuntimeError("GraphedDetector.batched_mask_logits: no batched call to take the rows from")
+        plan, ks = call
+        sizes = [int(n) for n in sizes]
+        if len(sizes) != len(ks):
+            raise ValueError(f"GraphedDetector.batched_mask_logits: {len(sizes)} sizes for a batch of {len(ks)}")
+        rows = torch.as_tensor(src_rows, dtype=torch.long).reshape(-1).cpu()
+        if rows.numel() != sum(sizes):
+            raise ValueError("GraphedDetector.batched_mask_logits: len(src_rows) != sum(sizes)")
+        shift = torch.repeat_interleave(torch.tensor([plan.kb - k for k in ks], dtype=torch.long),
+                                        torch.tensor(sizes, dtype=torch.long))
+        padded = (rows + shift).to(plan.img.device, non_blocking=True)
+        with torch.no_grad():
+            return self.model.mask_logits(plan.all_features, plan.memory, plan.hs_all, rows=(padded, sizes))
 
     def detect(self, samples, targets=None, prev_features=None):
         """The call itself: for segmentation models the graph already holds the forward without the mask head."""

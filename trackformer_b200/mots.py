@@ -3,9 +3,9 @@
 A mask's RLE is the dictionary pycocotools ``mask.encode(np.asfortranarray(mask))`` returns, ``{"size": [H, W],
 "counts": bytes}``: the run lengths of the mask read in column-major order, starting with a (possibly empty) run of
 zeros, written as pycocotools' ``rleToString`` characters.  ``encode`` / ``decode`` restate that format in numpy, so
-pycocotools is not needed; ``label_map_rle`` makes the RLEs of every track of a tracker label map at once, on the GPU
-(csrc/mask_rle.cu) for a CUDA map, so only the strings leave the device; ``write_results`` writes the file
-``MOTS20Sequence.write_results`` (datasets/tracking/mots20_sequence.py:72-91) writes, from bool masks or from RLEs.
+pycocotools is not needed; ``label_map_rle`` makes the RLEs of every track of a tracker label map at once
+(``label_maps_rle`` of several maps), on the GPU (csrc/mask_rle.cu) for CUDA maps, so only the strings leave the
+device; ``write_results`` writes the file ``MOTS20Sequence.write_results`` (datasets/tracking/mots20_sequence.py:72-91) writes, from bool masks or from RLEs.
 """
 import csv
 import os
@@ -13,7 +13,7 @@ import os
 import numpy as np
 import torch
 
-__all__ = ["encode", "decode", "decode_counts", "label_map_rle", "write_results"]
+__all__ = ["encode", "decode", "decode_counts", "label_map_rle", "label_maps_rle", "write_results"]
 
 _MAX_CHARS = 13                 # characters of any int64 count difference
 
@@ -85,20 +85,44 @@ def label_map_rle(label, ids) -> list:
     """RLEs of the masks ``label == ids[t]`` of a label map [H, W], in ``ids`` order (ids >= 0; other label values are
     background).  A CUDA int32 map is encoded by csrc/mask_rle.cu, and only the strings are copied to the host;
     anything else goes through ``encode``."""
-    if torch.is_tensor(label) and label.is_cuda and label.dtype == torch.int32:
+    return label_maps_rle([label], [ids])[0]
+
+
+def label_maps_rle(labels, ids_per_map) -> list:
+    """``label_map_rle`` of several label maps at once (e.g. one per sequence of a multi-sequence step; sizes may
+    differ): returns one list of RLEs per map.  When every map is a CUDA int32 tensor on one device, all of them are
+    encoded by ONE call of csrc/mask_rle.cu's batched entry (up to 16 maps per call) with two device-to-host copies,
+    the string offsets and the strings; otherwise each map goes through ``encode``."""
+    labels, ids_per_map = list(labels), [np.asarray(i, dtype=np.int64).reshape(-1) for i in ids_per_map]
+    if len(labels) != len(ids_per_map):
+        raise ValueError("label_maps_rle: one ids list per label map")
+    if any(len(i) and int(i.min()) < 0 for i in ids_per_map):
+        raise ValueError("label_map_rle: ids must be >= 0")
+    if not labels:
+        return []
+    first = labels[0]
+    if all(torch.is_tensor(lab) and lab.is_cuda and lab.dtype == torch.int32 and lab.device == first.device
+           for lab in labels):
         from . import ext
-        ids_t = torch.as_tensor(np.asarray(ids, dtype=np.int64).reshape(-1), dtype=torch.int32)
-        if ids_t.numel() and int(ids_t.min()) < 0:
-            raise ValueError("label_map_rle: ids must be >= 0")
-        h, w = (int(v) for v in label.shape)
-        strings = ext.load().mask_rle(label, ids_t.to(label.device))
-        return [{"size": [h, w], "counts": s} for s in strings]
+        packed = torch.from_numpy(np.concatenate(ids_per_map).astype(np.int32)).to(first.device, non_blocking=True)
+        views, o = [], 0
+        for i in ids_per_map:
+            views.append(packed[o:o + len(i)])
+            o += len(i)
+        out = []
+        for c in range(0, len(labels), 16):
+            strings = ext.load().mask_rle_batched(labels[c:c + 16], views[c:c + 16])
+            out += [[{"size": [int(v) for v in lab.shape], "counts": s} for s in per]
+                    for lab, per in zip(labels[c:c + 16], strings)]
+        return out
+    return [_label_map_rle_host(lab, ids) for lab, ids in zip(labels, ids_per_map)]
+
+
+def _label_map_rle_host(label, ids) -> list:
     lab = label.cpu().numpy() if torch.is_tensor(label) else np.asarray(label)
-    ids = [int(i) for i in np.asarray(ids).reshape(-1)]
+    ids = [int(i) for i in ids]
     if lab.ndim != 2:
         raise ValueError(f"label_map_rle: a 2-D label map is required, got shape {lab.shape}")
-    if any(i < 0 for i in ids):
-        raise ValueError("label_map_rle: ids must be >= 0")
     flat = np.ascontiguousarray(lab.T).reshape(-1)
     size = [int(lab.shape[0]), int(lab.shape[1])]
     return [{"size": size, "counts": _string(_counts(flat == i))} for i in ids]

@@ -16,8 +16,22 @@ Each sequence's results are those of a `DeviceTracker` over `GraphedDetector` on
 floating-point effects of running the detector at batch B.  `track_sequences` keeps up to `max_batch` sequences
 running and hands a finished sequence's slot to the next waiting one.
 
-Not batched (rejected in the constructor): segmentation masks (an `obj_detector_post` with "segm") and
-`generate_attention_maps=True`; `Tracker` and `DeviceTracker` keep both.
+Segmentation masks (MOTS: an `obj_detector_post` with "segm") and attention maps (`generate_attention_maps=True`,
+vanilla decoders) are batched too.  After the one read-back, word 7 of every result row names the query row whose mask
+and map its track takes, and then:
+
+  * per input-size group, ONE `batched_mask_logits` call runs the ragged mask head over the rows every sequence's
+    tracks took (the head stays eager);
+  * ONE launch of csrc/track_masks.cu resolves the label maps of every sequence, each against its own previous label
+    map for the tracks that keep their masks;
+  * with `mask_rle=True`, ONE call of csrc/mask_rle.cu's batched entry encodes every sequence's results (two
+    device-to-host copies); with bool masks all label maps leave the device in one copy;
+  * attention maps: one gather per group, copied to the host before the same synchronise.
+
+So a step synchronises the host at most three times whatever the number of sequences (result rows, then the RLE
+header and strings; twice with bool masks or maps alone), where stepping the sequences one by one costs up to three
+per sequence.  The detector must have `batched_mask_logits` for masks (a `GraphedDetector` over a segmentation model,
+or such a model, which is then wrapped) and a vanilla decoder for maps, as `Tracker` requires.
 """
 import ctypes
 
@@ -27,6 +41,8 @@ import torch
 from . import device_tracker
 from .device_tracker import DeviceTracker, _ArgsC, _MAX_ROWS
 from .graphed_detector import GraphedDetector
+from .mots import label_maps_rle
+from .segmentation import resolve_track_masks_many
 
 __all__ = ["MultiSequenceTracker", "track_sequences"]
 
@@ -55,12 +71,19 @@ class MultiSequenceTracker:
                  verbose=False, frame_ingest=None, mask_rle=False, max_batch=8):
         if not 1 <= int(max_batch) <= MAX_BATCH:
             raise ValueError(f"max_batch must be in 1..{MAX_BATCH}, got {max_batch}")
-        if "segm" in obj_detector_post:
-            raise ValueError("MultiSequenceTracker does not batch segmentation masks; use DeviceTracker or Tracker")
-        if generate_attention_maps:
-            raise ValueError("MultiSequenceTracker does not batch attention maps; use DeviceTracker or Tracker")
         if not callable(getattr(obj_detector, "batched", None)):
             obj_detector = GraphedDetector(obj_detector)
+        self.masks = "segm" in obj_detector_post
+        if self.masks and not (callable(getattr(obj_detector, "batched_mask_logits", None))
+                               and getattr(obj_detector, "has_mask_head", True)):
+            raise ValueError("MultiSequenceTracker does not batch segmentation masks; use DeviceTracker or Tracker")
+        self.generate_attention_maps = bool(generate_attention_maps)
+        if self.generate_attention_maps:
+            layers = getattr(getattr(getattr(obj_detector, "transformer", None), "decoder", None), "layers", None)
+            if not layers or not hasattr(layers[-1], "multihead_attn"):     # Tracker's check: a vanilla decoder
+                raise ValueError("MultiSequenceTracker does not batch attention maps; use DeviceTracker or Tracker")
+        if hasattr(obj_detector, "generate_attention_maps"):
+            obj_detector.generate_attention_maps = self.generate_attention_maps
         self.obj_detector = obj_detector
         self.obj_detector_post = obj_detector_post
         self.tracker_cfg = dict(tracker_cfg)
@@ -69,6 +92,7 @@ class MultiSequenceTracker:
         self._logger, self._verbose, self._mask_rle = logger, verbose, mask_rle
         self._seqs = {}
         self._result = self._host = None
+        self._pinned = {}                                    # name -> pinned host buffer, grown on demand
 
     @property
     def device(self):
@@ -82,8 +106,9 @@ class MultiSequenceTracker:
             from .frame_ingest import FrameIngest
             self.frame_ingest = FrameIngest(self.device)
         self._seqs[key] = DeviceTracker(self.obj_detector, self.obj_detector_post,
-                                        self.tracker_cfg if tracker_cfg is None else tracker_cfg, False, self._logger,
-                                        self._verbose, self.frame_ingest, self._mask_rle)
+                                        self.tracker_cfg if tracker_cfg is None else tracker_cfg,
+                                        self.generate_attention_maps, self._logger, self._verbose, self.frame_ingest,
+                                        self._mask_rle)
 
     def sequence(self, key):
         """The `DeviceTracker` holding sequence `key`'s state (`tracks`, `inactive_tracks`, `frame_index`, ...)."""
@@ -137,19 +162,19 @@ class MultiSequenceTracker:
                 blob["img"] = blob["img"].clone()
             groups.setdefault(tuple(blob["img"].shape[-2:]), []).append((key, blob))
 
-        order, keep = [], []
+        order, keep, calls = [], [], []
         for members in groups.values():
             seqs = [self._seqs[k] for k, _ in members]
             for seq in seqs:
                 seq._logger(f"FRAME: {seq.frame_index + 1}")
-            imgs = torch.cat([b["img"] for _, b in members]).to(dev)
+            imgs = torch.cat([b["img"] for _, b in members]).to(dev, non_blocking=True)
             targets = [{"track_query_boxes": s._bufs["q_boxes"][:s._n_query],
                         "track_query_hs_embeds": s._bufs["q_embeds"][:s._n_query]} if s._n_query else None
                        for s in seqs]
             out, features, ks, kb = self.obj_detector.batched(imgs, targets, [s._prev_features[0] for s in seqs])
             orig = torch.cat([b["orig_size"] for _, b in members])
             sizes = [tuple(int(v) for v in o) for o in orig.tolist()]
-            rows = self._rows(out, orig.to(dev)).float().contiguous()
+            rows = self._rows(out, orig.to(dev, non_blocking=True)).float().contiguous()
             hs = out["hs_embed"].float().contiguous()
             hidden, per_image = hs.shape[-1], kb + nq
             args = (_ArgsC * len(members))()
@@ -168,6 +193,8 @@ class MultiSequenceTracker:
                 seq._prev_features.append((features, i))
             self._launch(args, len(members), tensors)
             keep.append((rows, hs, args))                    # alive until the kernel has read them
+            calls.append((getattr(self.obj_detector, "last_batched", None), out.get("attention_maps"), ks, kb,
+                          range(len(order) - len(members), len(order))))
 
         # ---- the one read-back of the step: every sequence's header + result rows
         words = len(order) * stride
@@ -176,8 +203,125 @@ class MultiSequenceTracker:
         if host.is_pinned():
             torch.cuda.current_stream(dev).synchronize()
         out = host.numpy()
+        views = [out[p * stride:(p + 1) * stride] for p in range(len(order))]
+        bodies = [DeviceTracker._result_body(v) for v in views]
+        masks = self._resolve_all(order, bodies, calls) if self.masks else [None] * len(order)
+        maps = self._gather_maps(order, bodies, calls) if self.generate_attention_maps else None
+        synced = False
+        if self.masks:
+            masks, synced = self._mask_results(order, bodies, masks)
+        if maps is not None:
+            if not synced:                                   # no mask read-back waited for the copies above
+                self._synchronize(dev)
+            maps = [book() for book in maps]
         for p, (key, blob, (height, width)) in enumerate(order):
-            self._seqs[key]._take_results(out[p * stride:(p + 1) * stride], None, blob, height, width)
+            self._seqs[key]._take_results(views[p], None, blob, height, width, masks[p],
+                                          None if maps is None else maps[p])
+
+    # ------------------------------------------------------------------------------------- masks and maps, batched
+    @staticmethod
+    def _synchronize(dev):
+        if dev.type == "cuda":
+            torch.cuda.current_stream(dev).synchronize()
+
+    def _pinned_buffer(self, name, numel, dtype, dev):
+        """A host buffer of `numel` elements (pinned when the step runs on CUDA), reused across steps."""
+        buf = self._pinned.get(name)
+        if buf is None or buf.numel() < numel or buf.dtype != dtype:
+            buf = torch.empty(max(numel, 1), dtype=dtype)
+            if dev.type == "cuda":
+                buf = buf.pin_memory()
+            self._pinned[name] = buf
+        return buf[:numel]
+
+    def _resolve_all(self, order, bodies, calls):
+        """Every sequence's label map of this step: one ragged mask-head call per group, then one resolution launch.
+        Sets each sequence's `_label`; returns, per sequence, the label map (None when it has no active track)."""
+        jobs = [None] * len(order)
+        for p, (key, blob, orig) in enumerate(order):
+            body = bodies[p]
+            jobs[p] = self._seqs[key]._mask_job(body[:, 7].astype(np.int64), body[:, 0], blob, orig)
+        logits = [None] * len(order)
+        for call, _, _, _, members in calls:
+            sizes = [0 if jobs[p] is None else len(jobs[p][0]) for p in members]
+            rows = [r for p in members if jobs[p] is not None for r in jobs[p][0]]
+            if not rows:
+                continue
+            head = self.obj_detector.batched_mask_logits(rows, sizes, call)
+            o = 0
+            for p, n in zip(members, sizes):
+                if n:
+                    logits[p] = head[o:o + n]
+                o += n
+        work = []
+        for p, (key, blob, orig) in enumerate(order):
+            if jobs[p] is None:
+                continue
+            rows, src, prev, size = jobs[p]
+            lg = logits[p] if logits[p] is not None else torch.zeros(0, 1, 1, device=prev.device)
+            work.append((p, (lg, src, [int(i) for i in bodies[p][:, 0]], prev, size, size, orig)))
+        labels = resolve_track_masks_many([job for _, job in work])
+        out = [None] * len(order)
+        for (p, _), label in zip(work, labels):
+            out[p] = label
+        for p, (key, _, _) in enumerate(order):
+            self._seqs[key]._label = out[p]
+        return out
+
+    def _mask_results(self, order, bodies, labels):
+        """The results' masks of every sequence from its label map: RLEs from one batched encoder call, or bool arrays
+        from one copy of all label maps.  Also returns whether that read-back synchronised the host."""
+        live = [p for p, lab in enumerate(labels) if lab is not None]
+        out = [[] for _ in order]
+        if not live:
+            return out, False
+        dev = labels[live[0]].device
+        if self._mask_rle:
+            rles = label_maps_rle([labels[p] for p in live], [bodies[p][:, 0] for p in live])
+            for p, r in zip(live, rles):
+                out[p] = r
+            return out, dev.type == "cuda"
+        flat = torch.cat([labels[p].reshape(-1) for p in live])
+        host = self._pinned_buffer("labels", flat.numel(), torch.int32, dev)
+        host.copy_(flat, non_blocking=True)
+        self._synchronize(dev)
+        host = host.numpy()
+        o = 0
+        for p in live:
+            n = labels[p].numel()
+            lab = host[o:o + n].reshape(labels[p].shape)
+            out[p] = [lab == i for i in bodies[p][:, 0]]
+            o += n
+        return out, dev.type == "cuda"
+
+    def _gather_maps(self, order, bodies, calls):
+        """Issue one gather per group of the maps the tracks took and its copy to the host (no synchronise).  Returns
+        per sequence a callable that books its maps once the copies have landed."""
+        result = [None] * len(order)
+        for _, maps, ks, kb, members in calls:
+            flat = maps.flatten(0, 1)                        # [B * (kb + nq), h, w]: the padded rows of every image
+            per_image = maps.shape[1]
+            index, spans = [], []
+            for i, p in enumerate(members):
+                fresh = [int(r) for r in bodies[p][:, 7] if r >= 0]
+                spans.append((p, len(index), len(fresh)))
+                index += [i * per_image + kb - ks[i] + r for r in fresh]
+            host = None
+            if index:
+                index = torch.as_tensor(index, dtype=torch.long).to(flat.device, non_blocking=True)
+                picked = flat.index_select(0, index).float()
+                host = self._pinned_buffer(f"maps{members.start}", picked.numel(), torch.float32,
+                                           flat.device).view(picked.shape)
+                host.copy_(picked, non_blocking=True)
+            for p, o, n in spans:
+                seq = self._seqs[order[p][0]]
+                body = bodies[p]
+
+                def book(seq=seq, body=body, host=host, o=o, n=n):
+                    return seq._book_maps(body[:, 7].astype(np.int64), body[:, 0],
+                                          None if not n else host[o:o + n].numpy().copy())   # buffer is reused
+                result[p] = book
+        return result
 
 
 def track_sequences(tracker, sequences):

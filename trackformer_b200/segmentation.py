@@ -19,6 +19,7 @@ from __future__ import annotations
 
 from typing import List, Optional
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 from torch import Tensor, nn
@@ -429,14 +430,48 @@ def resolve_track_masks(logits: Tensor, src, ids, prev_label: Optional[Tensor], 
     pixel labelled with the first track of maximal value if that value exceeds 0.5 (models/tracker.py:509-521).
 
     On CUDA fp32 logits this is one launch of csrc/track_masks.cu; otherwise the reference's torch ops."""
+    return resolve_track_masks_many([(logits, src, ids, prev_label, size, crop, orig)])[0]
+
+
+def resolve_track_masks_many(jobs) -> List[Tensor]:
+    """``resolve_track_masks`` of several frames (e.g. one per sequence of a multi-sequence step): ``jobs`` is a list
+    of its argument tuples ``(logits, src, ids, prev_label, size, crop, orig)``; returns their label maps in order.
+
+    When every job's logits are CUDA fp32 on one device, all of them are ONE launch of csrc/track_masks.cu (up to 16
+    per launch), each label map equal bit for bit to its own call; otherwise each job takes the reference's torch ops."""
+    jobs = list(jobs)
+    if not jobs:
+        return []
+    dev = jobs[0][0].device
+    if all(j[0].is_cuda and j[0].dtype == torch.float32 and j[0].device == dev for j in jobs):
+        srcs, idss = [], []
+        for _, src, ids, *_ in jobs:
+            srcs.append(torch.as_tensor(src, dtype=torch.int32).reshape(-1).cpu().numpy())
+            idss.append(torch.as_tensor(ids, dtype=torch.int32).reshape(-1).cpu().numpy())
+        packed = torch.from_numpy(np.concatenate(srcs + idss).astype(np.int32)).to(dev, non_blocking=True)
+        views, o = [], 0
+        for a in srcs + idss:
+            views.append(packed[o:o + len(a)])
+            o += len(a)
+        n = len(jobs)
+        out = []
+        for c in range(0, n, 16):
+            part = range(c, min(c + 16, n))
+            out += ext.load().track_masks_batched(
+                [jobs[i][0].contiguous() for i in part], [views[i] for i in part], [views[n + i] for i in part],
+                [None if jobs[i][3] is None else jobs[i][3].to(device=dev, dtype=torch.int32) for i in part],
+                [[int(jobs[i][4][0]), int(jobs[i][4][1]), int(jobs[i][5][0]), int(jobs[i][5][1]),
+                  int(jobs[i][6][0]), int(jobs[i][6][1])] for i in part])
+        return out
+    return [_resolve_track_masks_host(*job) for job in jobs]
+
+
+def _resolve_track_masks_host(logits: Tensor, src, ids, prev_label: Optional[Tensor], size, crop, orig) -> Tensor:
+    """``resolve_track_masks`` with the reference's torch ops (any device and dtype)."""
     H, W = (int(v) for v in orig)
     src = torch.as_tensor(src, dtype=torch.int32).reshape(-1)
     ids = torch.as_tensor(ids, dtype=torch.int32).reshape(-1)
     dev = logits.device
-    if logits.is_cuda and logits.dtype == torch.float32:
-        prev = None if prev_label is None else prev_label.to(device=dev, dtype=torch.int32)
-        return ext.load().track_masks(logits.contiguous(), src.to(dev), ids.to(dev), prev, int(size[0]), int(size[1]),
-                                      int(crop[0]), int(crop[1]), H, W)
     if len(ids) == 0:
         return torch.full((H, W), -1, dtype=torch.int32, device=dev)
     fresh = src >= 0

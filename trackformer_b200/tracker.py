@@ -248,6 +248,11 @@ class Tracker:
         if fresh:
             rows = torch.as_tensor([int(src_rows[k]) for k in fresh], dtype=torch.long).to(maps.device)
             host = maps.index_select(0, rows).float().cpu().numpy()
+        return self._book_maps(src_rows, ids, host)
+
+    def _book_maps(self, src_rows, ids, host):
+        """Keep this frame's maps: `host` [n, h, w] holds the new maps of the tracks with `src_rows[t] >= 0`, in order;
+        the other tracks keep theirs.  Returns the maps in `ids` order (None for a track that never had one)."""
         new, j = {}, 0
         for k, tid in enumerate(ids):
             tid = int(tid)
@@ -298,13 +303,13 @@ class Tracker:
         masks = det_out[0]["pred_masks"][0]           # any reference-shaped detector: the full head's output
         return masks.index_select(0, torch.as_tensor(rows, dtype=torch.long, device=masks.device))
 
-    def _resolve_masks(self, det_out, src_rows, ids, blob, orig):
-        """Masks of the active tracks (ids, in list order) of this frame: `src_rows[t]` is the query row whose mask
-        track t takes, -1 to keep its previous one.  Returns the results' masks in `ids` order: bool arrays [H, W] from
-        the host label map (the one read-back), or with `mask_rle` the COCO RLEs made from the device label map."""
+    def _mask_job(self, src_rows, ids, blob, orig):
+        """What resolving this frame's masks takes, for the active tracks `ids` (list order) with `src_rows[t]` the query
+        row whose mask track t takes (-1: it keeps its previous one): `(rows, src, prev, size)` -- the sorted query rows
+        the mask head must compute, each track's index into them (-1 when stale), the previous label map when a track
+        is stale (else None) and the padded input size.  None when no track is active."""
         if not len(ids):
-            self._label = None
-            return []
+            return None
         stale = any(r < 0 for r in src_rows)
         if stale and (self._label is None or tuple(self._label.shape) != tuple(orig)):
             # the reference fails here too (torch.stack of masks of different sizes, tracker.py:510)
@@ -313,17 +318,26 @@ class Tracker:
         rows = sorted({int(r) for r in src_rows if r >= 0})
         index = {r: i for i, r in enumerate(rows)}
         src = [index[int(r)] if r >= 0 else -1 for r in src_rows]
+        size = [int(v) for v in blob["size"].reshape(-1, 2)[0].tolist()]
+        return rows, src, (self._label if stale else None), size
+
+    def _resolve_masks(self, det_out, src_rows, ids, blob, orig):
+        """Masks of the active tracks (ids, in list order) of this frame: `src_rows[t]` is the query row whose mask
+        track t takes, -1 to keep its previous one.  Returns the results' masks in `ids` order: bool arrays [H, W] from
+        the host label map (the one read-back), or with `mask_rle` the COCO RLEs made from the device label map."""
+        job = self._mask_job(src_rows, ids, blob, orig)
+        if job is None:
+            self._label = None
+            return []
+        rows, src, prev, size = job
         if rows:
             logits = self._mask_rows(det_out, rows)
         else:
             logits = torch.zeros(0, 1, 1, device=self._label.device)
-        size = [int(v) for v in blob["size"].reshape(-1, 2)[0].tolist()]
-        label = resolve_track_masks(logits, src, [int(i) for i in ids], self._label if stale else None, size, size,
-                                    orig)
-        self._label = label
+        self._label = resolve_track_masks(logits, src, [int(i) for i in ids], prev, size, size, orig)
         if self.mask_rle:
-            return label_map_rle(label, ids)
-        host = label.cpu().numpy()
+            return label_map_rle(self._label, ids)
+        host = self._label.cpu().numpy()
         return [host == i for i in ids]
 
     def _take_slot(self):
