@@ -470,6 +470,36 @@ int tfb200_mot_eval_f32(const int64_t* seq, const int32_t* frame_obj, const int3
                         int64_t n_trk, int64_t tp_cells, int max_obj, int max_hyp, int64_t pair_cap, void* workspace,
                         size_t workspace_bytes, int64_t* out, void* stream);
 
+/* MOTS metrics of S sequences at once (csrc/mots_eval.cu, csrc/mots_eval_core.h): the pairs of tfb200_mot_eval_f32
+ * from masks given as COCO RLE counts strings (pycocotools rleToString), then its matching unchanged.  seq [S][8] as
+ * tfb200_mot_eval_f32's; seq_hw [S][2] int32 the sequence's H, W (H x W < 2^28).  F frames over all sequences in
+ * order; frame_mask int32 [3F + 1]: frame f's GT masks are rows frame_mask[3f] .., its ignore regions frame_mask[3f +
+ * 1] .., its hypotheses frame_mask[3f + 2] .. frame_mask[3f + 3]; frame_cell int64 [F + 1] the prefix sums of (GT
+ * masks + 1) x hypotheses per frame (cells = the total); frame_obj int32 [F + 1] the prefix sums of GT masks, obj_id
+ * [n_obj] their dense GT ids.  mask [n_masks][4] int32 = {frame, dense id (GT id, track id or 0), H, W}; mask k's
+ * string is chars[str_off[k] .. str_off[k + 1]) (str_off int64 [n_masks + 1]).  interval_cap >= the sum over masks
+ * of floor(string length / 2), < 2^31; pair_cap >= min(sum of GT x hypotheses per frame, 2 x GT masks) (a GT mask
+ * has at most two partners with IoU >= 0.5 when hypotheses do not overlap).  A pair is valid when its pixel counts
+ * give inter > 0 and 2 inter >= union, with d = 1 - inter / union; a hypothesis with no valid pair and 2 |h & ignore| >
+ * |h| is removed.  Writes out [S][16] as tfb200_mot_eval_f32 (hypotheses = the kept ones) followed by [S][11] =
+ * {status, GT masks, kept hypotheses, removed hypotheses, intervals, intersecting (GT, hypothesis) pairs, then the
+ * first sequence-local frame of status bits 1, 2, 4, 8, 16 (INT64_MAX when unset)}.  status bit 1: GT masks or ignore
+ * regions of a frame overlap; 2: hypotheses of a frame overlap; 4: a mask whose size differs from its sequence's (or
+ * H x W out of range); 8: a malformed string (a character outside '0' .. 'o', a value cut short or of more than 7
+ * characters, a negative count) or runs that do not cover H x W; 16: more intervals than interval_cap (nothing is
+ * decoded).  A bad mask contributes no pixels; a set bit leaves the sequence's counts meaningless.  Workspace:
+ * tfb200_mots_eval_workspace_bytes(...) (0 for bad sizes), about 32 B per interval of interval_cap plus 4 B per cell
+ * and tfb200_mot_eval_f32's.  Integer counts are exact and every output is the same run to run.  Sizes out of range:
+ * TFB200_E_SHAPE.                                                                                                  */
+size_t tfb200_mots_eval_workspace_bytes(int S, int F, int n_masks, int64_t n_gt, int64_t n_trk, int64_t tp_cells,
+                                        int max_obj, int max_hyp, int64_t pair_cap, int64_t interval_cap,
+                                        int64_t cells);
+int tfb200_mots_eval(const int64_t* seq, const int32_t* seq_hw, const int32_t* frame_mask, const int64_t* frame_cell,
+                     const int32_t* frame_obj, const int32_t* obj_id, const int32_t* mask, const int64_t* str_off,
+                     const uint8_t* chars, int S, int F, int n_masks, int64_t n_gt, int64_t n_trk, int64_t tp_cells,
+                     int max_obj, int max_hyp, int64_t pair_cap, int64_t interval_cap, int64_t cells, void* workspace,
+                     size_t workspace_bytes, int64_t* out, void* stream);
+
 /* COCO box / mask AP (csrc/coco_eval.cu; what pycocotools 2.0's COCOeval computes for the reference's CocoEvaluator,
  * datasets/coco_eval.py).  tfb200_coco_match_f32 evaluates the B images of one update.  img [B][10] int64 = {GT image
  * row, first detection row, detection count, H, W, device address of the image's masks uint8/bool [n][H][W] (segm),

@@ -5,7 +5,8 @@ A mask's RLE is the dictionary pycocotools ``mask.encode(np.asfortranarray(mask)
 zeros, written as pycocotools' ``rleToString`` characters.  ``encode`` / ``decode`` restate that format in numpy, so
 pycocotools is not needed; ``label_map_rle`` makes the RLEs of every track of a tracker label map at once
 (``label_maps_rle`` of several maps), on the GPU (csrc/mask_rle.cu) for CUDA maps, so only the strings leave the
-device; ``write_results`` writes the file ``MOTS20Sequence.write_results`` (datasets/tracking/mots20_sequence.py:72-91) writes, from bool masks or from RLEs.
+device; ``write_results`` writes the file ``MOTS20Sequence.write_results`` (datasets/tracking/mots20_sequence.py:72-91) writes, from bool masks or from RLEs,
+and ``load_results`` reads such a file (or a MOTS20 GT file) back with the masks kept as RLEs.
 """
 import csv
 import os
@@ -13,7 +14,8 @@ import os
 import numpy as np
 import torch
 
-__all__ = ["encode", "decode", "decode_counts", "label_map_rle", "label_maps_rle", "write_results"]
+__all__ = ["encode", "decode", "decode_counts", "label_map_rle", "label_maps_rle", "read_rows", "load_results",
+           "write_results"]
 
 _MAX_CHARS = 13                 # characters of any int64 count difference
 
@@ -126,6 +128,35 @@ def _label_map_rle_host(label, ids) -> list:
     flat = np.ascontiguousarray(lab.T).reshape(-1)
     size = [int(lab.shape[0]), int(lab.shape[1])]
     return [{"size": size, "counts": _string(_counts(flat == i))} for i in ids]
+
+
+def read_rows(path: str) -> list:
+    """The rows of a MOTS20 text file (results or ``gt/gt.txt``) in file order: ``(frame, id, class_id, rle)`` with the
+    file's 1-based frame and id.  A duplicate (frame, id) raises ``ValueError``."""
+    rows, seen = [], set()
+    with open(path, newline="") as f:
+        for n, fields in enumerate(csv.reader(f, delimiter=" "), 1):
+            if not fields:
+                continue
+            if len(fields) != 6:
+                raise ValueError(f"{path}:{n}: a MOTS20 row has 6 fields (frame id class H W counts)")
+            frame, i, cls, h, w = (int(v) for v in fields[:5])
+            if (frame, i) in seen:
+                raise ValueError(f"{path}: frame {frame}: duplicate id {i}")
+            seen.add((frame, i))
+            rows.append((frame, i, cls, {"size": [h, w], "counts": fields[5].encode()}))
+    return rows
+
+
+def load_results(path: str) -> dict:
+    """A MOTS20 text file as ``{id - 1: {frame - 1: {"mask": RLE dict, "class_id": class}}}``, ids in the order they
+    first appear: what ``MOTS20Sequence.load_results`` returns (datasets/tracking/mots20_sequence.py:93-124), with the
+    mask kept as its RLE and every class kept.  ``write_results`` of it rewrites a results file byte for byte.  Reads
+    GT files too.  A duplicate (frame, id) raises ``ValueError``."""
+    out = {}
+    for frame, i, cls, rle in read_rows(path):
+        out.setdefault(i - 1, {})[frame - 1] = {"mask": rle, "class_id": cls}
+    return out
 
 
 def write_results(results: dict, output_dir: str, seq_name: str) -> str:
