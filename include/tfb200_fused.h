@@ -84,6 +84,37 @@ int tfb200_sampling_prep_bwd_f32(const float* grad_loc, const float* grad_attn, 
  * or 2 (infeasible: a box whose costs are all +inf).  Double-precision duals, like scipy.                           */
 int tfb200_lsa_f32(const float* cost, const int* offsets_dev, int64_t* src, int64_t* tgt, int K, int B, int Q, int T,
                    int max_targets, int* status_dev, void* stream);
+/* Shared memory tfb200_lsa_f32 needs for Q queries and max_targets boxes per image; it refuses problems needing more
+ * than TFB200_LSA_SHARED_MAX bytes (about 8,000 queries), which tfb200_lsa_wide_f32 takes.                         */
+#define TFB200_LSA_SHARED_MAX (200 * 1024)
+size_t tfb200_lsa_shared_bytes(int Q, int max_targets);
+/* tfb200_lsa_f32 for problems too wide for its shared-memory state (it refuses above about 8,000 queries): the same
+ * shortest-augmenting-path solver, tie rule, outputs and status codes, with each problem's cost block transposed to
+ * [target][query] and its column state kept in a caller-provided device workspace of
+ * tfb200_lsa_wide_workspace_bytes(K, B, Q, max_targets) bytes (about 4 * Q * max_targets + 25 * Q per problem).  On
+ * every problem tfb200_lsa_f32 accepts it returns the same src / tgt.  Two launches (transpose, solve).              */
+size_t tfb200_lsa_wide_workspace_bytes(int K, int B, int Q, int max_targets);
+int tfb200_lsa_wide_f32(const float* cost, const int* offsets_dev, int64_t* src, int64_t* tgt, int K, int B, int Q,
+                        int T, int max_targets, void* workspace, size_t workspace_bytes, int* status_dev, void* stream);
+
+/* Two-stage Deformable DETR (deformable_transformer.py:77-122, 180-194; csrc/two_stage_core.h).
+ * proposals: for every token (b, s) of the L levels hw = {H0, W0, H1, W1, ...} (sum H*W = S, L <= 8), with valid W / H
+ * the unpadded entries of the level's first mask row / column (mask [B][S] uint8, nonzero = padded; NULL = none):
+ * prop [B][S][4] = log(p / (1 - p)) of p = ((x+.5)/W_valid, (y+.5)/H_valid, .05*2^l, .05*2^l), or +inf unless the token
+ * is unpadded and all four p lie in (0.01, 0.99); valid [B][S] = that flag; with memory [B][S][C] (C % 4 == 0),
+ * masked = memory with the invalid rows zeroed.  One launch.
+ * mask_rows: y = x * valid per row of [rows][C] (C % 4 == 0): the masking alone, and its gradient.  One launch.
+ * memory / masked / x / y are read and written as float4: 16-byte aligned (TFB200_E_SHAPE otherwise).
+ * select: per image the k largest logits[b][s][0] over s (ties: lower s first), best first -> index [B][k]; boxes
+ * [B][k][4] = unact[b][index]; ref = sigmoid(boxes); embed [B][k][512]: element c*128 + j = sin (j even) or cos (j odd)
+ * of sigmoid(boxes[c]) * 2pi / dim_t[j] (dim_t [128] as torch computes it).  keys: [B][S] uint32 workspace.
+ * k <= min(S, 2048).  One launch, no host synchronisation.                                                          */
+int tfb200_two_stage_proposals_f32(const uint8_t* mask, const float* memory, float* masked, float* prop,
+                                   uint8_t* valid, int B, int S, int L, int C, const int* hw, void* stream);
+int tfb200_two_stage_mask_rows_f32(const float* x, const uint8_t* valid, float* y, int64_t rows, int C, void* stream);
+int tfb200_two_stage_select_f32(const float* logits, const float* unact, const float* dim_t, uint32_t* keys,
+                                int64_t* index, float* boxes, float* ref, float* embed, int B, int S, int C, int k,
+                                void* stream);
 
 /* Detection post-processing for the online tracker (deformable_detr.py:286-334 + the per-track read-backs of
  * tracker.py:306-330): logits [N][Q][C], boxes [N][Q][4] (cx, cy, w, h normalised), sizes_hw [N][2] int64 (h, w) on the

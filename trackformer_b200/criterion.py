@@ -4,6 +4,9 @@ Mirror of ``SetCriterion`` (src/trackformer/models/detr.py:139-443) for the loss
 TrackFormer configs use -- ``labels`` (sigmoid focal or weighted cross-entropy), ``boxes`` (L1 + GIoU) and
 ``cardinality`` (logging only) -- applied to the last decoder layer and to every auxiliary layer with its own
 Hungarian matching, normalised by the world-averaged number of boxes (one scalar all-reduce, :399-401).
+Two-stage models add ``enc_outputs``, the encoder proposals scored against class-agnostic targets (every label 0)
+with their own matching (:425-441), under ``_enc`` keys; on CUDA that is one matching-cost launch, the workspace
+Hungarian solver (every memory token is a query) and one pass of the fused loss, with no host synchronisation.
 ``masks`` (sigmoid focal + dice on the bilinearly upsampled mask logits, :330-357) applies to the last layer only;
 on CUDA fp32 it is csrc/mask_head.cu, which samples the low-resolution logits at every target pixel on the fly
 instead of materialising the upsampled masks.
@@ -273,7 +276,53 @@ class SetCriterion(nn.Module):
                 kw = {"log": False} if name == "labels" else {}
                 part = self.get_loss(name, aux, targets, all_indices[i + 1], num_boxes, **kw)
                 losses.update({f"{k}_{i}": v for k, v in part.items()})
+        if "enc_outputs" in outputs:
+            losses.update(self._encoder_losses_host(outputs["enc_outputs"], targets, num_boxes))
         return losses, indices
+
+    @staticmethod
+    def _binary_targets(targets):
+        """the targets with every label 0 (detr.py:427-429; only boxes and labels are read)"""
+        return [{"boxes": t["boxes"], "labels": torch.zeros_like(t["labels"])} for t in targets]
+
+    def _encoder_losses_host(self, enc_outputs, targets, num_boxes):
+        """the ``_enc`` losses of detr.py:425-441: the matcher and the loss functions on class-agnostic targets"""
+        bin_targets = self._binary_targets(targets)
+        indices = self.matcher(enc_outputs, bin_targets)
+        losses = {}
+        for name in self.losses:
+            if name == "masks":
+                continue
+            kw = {"log": False} if name == "labels" else {}
+            part = self.get_loss(name, enc_outputs, bin_targets, indices, num_boxes, **kw)
+            losses.update({f"{k}_enc": v for k, v in part.items()})
+        return losses
+
+    def _encoder_losses(self, enc_logits, enc_boxes, targets, num_boxes):
+        """``_encoder_losses_host`` for stacked callers; on CUDA fp32 one ``match_cost`` + ``lsa`` (the workspace solver:
+        every token is a query) and one K = 1 pass of the fused loss, nothing read back."""
+        bin_targets = self._binary_targets(targets)
+        sizes = [len(t["labels"]) for t in targets]
+        match = None
+        if (self.device_matcher and _FUSED_LOSS and enc_logits.dtype == torch.float32
+                and hasattr(self.matcher, "match_layers_device")
+                and set(self.losses) - {"masks"} == {"labels", "boxes", "cardinality"}):
+            match = self.matcher.match_layers_device(enc_logits.detach()[None], enc_boxes.detach()[None], bin_targets)
+        if match is None:
+            if num_boxes is None:
+                num_boxes = self._num_boxes(targets, enc_logits.device)
+            return self._encoder_losses_host({"pred_logits": enc_logits, "pred_boxes": enc_boxes}, targets, num_boxes)
+        src2d, tgt2d, status = match
+        torch._assert_async(status[0] == 0)
+        dev = enc_logits.device
+        key = ("n_gt", tuple(sizes), dev)
+        n_gt = self._index_memo.get(key)
+        if n_gt is None:
+            n_gt = self._index_memo[key] = torch.as_tensor(sizes, dtype=torch.float, device=dev)
+        if num_boxes is None:
+            num_boxes = self._num_boxes(targets, dev)
+        fused = self._fused_losses(enc_logits[None], enc_boxes[None], src2d, tgt2d, bin_targets, sizes, n_gt, num_boxes)
+        return {f"{k}_enc": fused[k] for k in ("loss_ce", "loss_bbox", "loss_giou", "cardinality_error")}
 
     @staticmethod
     def _matched_of(indices, targets, device):
@@ -352,7 +401,8 @@ class SetCriterion(nn.Module):
         losses.stacked = (ce, l1, gi)
         return losses
 
-    def forward_stacked(self, logits, boxes, targets, num_boxes=None, pred_masks=None, track_queries=False):
+    def forward_stacked(self, logits, boxes, targets, num_boxes=None, pred_masks=None, track_queries=False,
+                        enc_outputs=None):
         """Same losses as ``forward`` for a detector whose K decoder layers arrive stacked --
         ``logits [K,B,Q,C]``, ``boxes [K,B,Q,4]``, last layer = final prediction -- computed in ONE pass over
         all layers instead of K passes (the reference loops, detr.py:404-424): one Hungarian transfer, one focal
@@ -369,7 +419,16 @@ class SetCriterion(nn.Module):
 
         Both classifiers take this pass: the sigmoid focal loss (``focal_loss``) and the weighted cross-entropy of the
         softmax classifier, whose false-positive track queries keep their full weight when ``tracking`` and
-        ``track_query_false_positive_eos_weight`` are set (detr.py:190-197)."""
+        ``track_query_false_positive_eos_weight`` are set (detr.py:190-197).
+
+        ``enc_outputs = (logits [B,S,C], boxes [B,S,4])`` of a two-stage model's encoder head adds the ``_enc`` losses of
+        ``forward`` (see ``_encoder_losses``)."""
+        losses = self._forward_stacked(logits, boxes, targets, num_boxes, pred_masks, track_queries, enc_outputs)
+        if enc_outputs is not None and not any(k.endswith("_enc") for k in losses):
+            losses.update(self._encoder_losses(enc_outputs[0], enc_outputs[1], targets, num_boxes))
+        return losses
+
+    def _forward_stacked(self, logits, boxes, targets, num_boxes, pred_masks, track_queries, enc_outputs):
         k, bs, nq, _ = logits.shape
         layers = [{"pred_logits": logits[i], "pred_boxes": boxes[i]} for i in range(k)]
         with_masks = "masks" in self.losses
@@ -387,6 +446,8 @@ class SetCriterion(nn.Module):
             if with_masks and pred_masks is not None:
                 out["pred_masks"] = pred_masks
             out["aux_outputs"] = layers[:-1]
+            if enc_outputs is not None:
+                out["enc_outputs"] = {"pred_logits": enc_outputs[0], "pred_boxes": enc_outputs[1]}
             if not with_masks:
                 return self.forward(out, targets, num_boxes)
             found, indices = self._forward(out, targets, num_boxes, masks=pred_masks is not None)

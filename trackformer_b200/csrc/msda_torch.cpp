@@ -706,11 +706,125 @@ std::vector<at::Tensor> lsa(const at::Tensor& cost, const at::Tensor& offsets, i
   auto iopt = c.options().dtype(at::kLong);
   at::Tensor src = at::zeros({K, T}, iopt), tgt = at::zeros({K, T}, iopt);
   at::Tensor status = at::zeros({1}, c.options().dtype(at::kInt));
-  const int rc = tfb200_lsa_f32(c.data_ptr<float>(), offsets.data_ptr<int>(), src.data_ptr<int64_t>(), tgt.data_ptr<int64_t>(),
-                                int(K), int(B), int(Q), int(T), int(max_targets), status.data_ptr<int>(),
-                                c10::cuda::getCurrentCUDAStream().stream());
+  // the workspace solver takes exactly the problems the shared-memory solver refuses for their size
+  int rc;
+  if (max_targets > 0 && max_targets <= Q &&
+      tfb200_lsa_shared_bytes(int(Q), int(max_targets)) > TFB200_LSA_SHARED_MAX) {
+    at::Tensor ws = at::empty({int64_t(tfb200_lsa_wide_workspace_bytes(int(K), int(B), int(Q), int(max_targets)))},
+                              c.options().dtype(at::kByte));
+    rc = tfb200_lsa_wide_f32(c.data_ptr<float>(), offsets.data_ptr<int>(), src.data_ptr<int64_t>(), tgt.data_ptr<int64_t>(),
+                             int(K), int(B), int(Q), int(T), int(max_targets), ws.data_ptr(), size_t(ws.numel()),
+                             status.data_ptr<int>(), c10::cuda::getCurrentCUDAStream().stream());
+  } else {
+    rc = tfb200_lsa_f32(c.data_ptr<float>(), offsets.data_ptr<int>(), src.data_ptr<int64_t>(), tgt.data_ptr<int64_t>(),
+                        int(K), int(B), int(Q), int(T), int(max_targets), status.data_ptr<int>(),
+                        c10::cuda::getCurrentCUDAStream().stream());
+  }
   TORCH_CHECK(rc == 0, "lsa failed (code ", rc, ")");
   return {src, tgt, status};
+}
+
+// lsa on the workspace solver whatever the size (tests compare it with the shared-memory one)
+std::vector<at::Tensor> lsa_wide(const at::Tensor& cost, const at::Tensor& offsets, int64_t max_targets) {
+  TORCH_CHECK(cost.is_cuda() && cost.scalar_type() == at::kFloat && cost.dim() == 4, "lsa_wide: cost must be a [K,B,Q,T] fp32 CUDA tensor");
+  TORCH_CHECK(offsets.is_cuda() && offsets.scalar_type() == at::kInt && offsets.numel() == cost.size(1) + 1,
+              "lsa_wide: offsets must be an int32 CUDA tensor of B+1 entries");
+  const at::Tensor c = cost.contiguous();
+  const c10::cuda::CUDAGuard guard(cost.device());
+  const int64_t K = c.size(0), B = c.size(1), Q = c.size(2), T = c.size(3);
+  auto iopt = c.options().dtype(at::kLong);
+  at::Tensor src = at::zeros({K, T}, iopt), tgt = at::zeros({K, T}, iopt);
+  at::Tensor status = at::zeros({1}, c.options().dtype(at::kInt));
+  const size_t bytes = tfb200_lsa_wide_workspace_bytes(int(K), int(B), int(Q), int(max_targets));
+  at::Tensor ws = at::empty({int64_t(std::max<size_t>(bytes, 1))}, c.options().dtype(at::kByte));
+  const int rc = tfb200_lsa_wide_f32(c.data_ptr<float>(), offsets.data_ptr<int>(), src.data_ptr<int64_t>(),
+                                     tgt.data_ptr<int64_t>(), int(K), int(B), int(Q), int(T), int(max_targets), ws.data_ptr(),
+                                     bytes, status.data_ptr<int>(), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "lsa_wide failed (code ", rc, ")");
+  return {src, tgt, status};
+}
+
+// ---- two-stage Deformable DETR (csrc/two_stage.cu) --------------------------------------------------------------------
+// the kernels read and write rows as float4: a contiguous view at an offset that is not a multiple of 4 floats is copied
+static at::Tensor aligned16(const at::Tensor& t) {
+  const at::Tensor c = t.contiguous();
+  return (reinterpret_cast<uintptr_t>(c.data_ptr()) & 15u) == 0 ? c : c.clone();
+}
+
+// -> {prop [B,S,4], valid uint8 [B,S], masked memory [B,S,C] (empty without memory)}, on CUDA device `device_index`
+std::vector<at::Tensor> two_stage_proposals(const c10::optional<at::Tensor>& mask, const c10::optional<at::Tensor>& memory,
+                                            const std::vector<int64_t>& hw, int64_t batch, int64_t device_index) {
+  TORCH_CHECK(hw.size() % 2 == 0 && !hw.empty() && hw.size() <= 16, "two_stage_proposals: hw = [H0, W0, H1, W1, ...], <= 8 levels");
+  std::vector<int> hw32(hw.begin(), hw.end());
+  int64_t S = 0;
+  for (size_t l = 0; l < hw.size(); l += 2) S += hw[l] * hw[l + 1];
+  TORCH_CHECK(device_index >= 0 && device_index < c10::cuda::device_count(), "two_stage_proposals: no CUDA device ",
+              device_index);
+  const at::Device dev(at::kCUDA, c10::DeviceIndex(device_index));
+  at::Tensor mk, mem;
+  if (mask.has_value() && mask->defined()) {
+    mk = mask->contiguous();
+    TORCH_CHECK(mk.is_cuda() && mk.element_size() == 1 && mk.dim() == 2 && mk.size(0) == batch && mk.size(1) == S,
+                "two_stage_proposals: mask must be a [B,S] bool / uint8 CUDA tensor");
+    TORCH_CHECK(mk.device() == dev, "two_stage_proposals: mask on ", mk.device(), ", expected ", dev);
+  }
+  int64_t C = 0;
+  if (memory.has_value() && memory->defined()) {
+    mem = aligned16(*memory);
+    TORCH_CHECK(mem.is_cuda() && mem.scalar_type() == at::kFloat && mem.dim() == 3 && mem.size(0) == batch && mem.size(1) == S,
+                "two_stage_proposals: memory must be a [B,S,C] fp32 CUDA tensor");
+    TORCH_CHECK(mem.device() == dev, "two_stage_proposals: memory on ", mem.device(), ", expected ", dev);
+    C = mem.size(2);
+  }
+  const c10::cuda::CUDAGuard guard(dev);
+  auto fopt = at::TensorOptions().device(dev).dtype(at::kFloat);
+  at::Tensor prop = at::empty({batch, S, 4}, fopt), valid = at::empty({batch, S}, fopt.dtype(at::kByte));
+  at::Tensor masked = mem.defined() ? at::empty_like(mem) : at::Tensor();
+  const int rc = tfb200_two_stage_proposals_f32(mk.defined() ? static_cast<const uint8_t*>(mk.data_ptr()) : nullptr,
+                                                mem.defined() ? mem.data_ptr<float>() : nullptr,
+                                                masked.defined() ? masked.data_ptr<float>() : nullptr, prop.data_ptr<float>(),
+                                                valid.data_ptr<uint8_t>(), int(batch), int(S), int(hw.size() / 2), int(C),
+                                                hw32.data(), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "two_stage_proposals failed (code ", rc, ")");
+  return {prop, valid, masked.defined() ? masked : at::empty({0}, fopt)};
+}
+
+at::Tensor two_stage_mask_rows(const at::Tensor& x, const at::Tensor& valid) {
+  TORCH_CHECK(x.is_cuda() && x.scalar_type() == at::kFloat && valid.is_cuda() && valid.scalar_type() == at::kByte,
+              "two_stage_mask_rows: fp32 rows and uint8 flags on CUDA");
+  TORCH_CHECK(x.device() == valid.device(), "two_stage_mask_rows: rows on ", x.device(), ", flags on ", valid.device());
+  const at::Tensor xc = aligned16(x), vc = valid.contiguous();
+  const int64_t C = xc.size(-1), rows = xc.numel() / std::max<int64_t>(C, 1);
+  TORCH_CHECK(vc.numel() == rows, "two_stage_mask_rows: one flag per row");
+  const c10::cuda::CUDAGuard guard(x.device());
+  at::Tensor y = at::empty_like(xc);
+  const int rc = tfb200_two_stage_mask_rows_f32(xc.data_ptr<float>(), vc.data_ptr<uint8_t>(), y.data_ptr<float>(), rows, int(C),
+                                                c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "two_stage_mask_rows failed (code ", rc, ")");
+  return y;
+}
+
+// -> {index int64 [B,k], boxes [B,k,4] (unactivated), ref [B,k,4], embed [B,k,512]}
+std::vector<at::Tensor> two_stage_select(const at::Tensor& logits, const at::Tensor& unact, const at::Tensor& dim_t, int64_t k) {
+  TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == at::kFloat && logits.dim() == 3 && unact.scalar_type() == at::kFloat &&
+              unact.dim() == 3 && unact.size(2) == 4 && unact.size(0) == logits.size(0) && unact.size(1) == logits.size(1) &&
+              dim_t.scalar_type() == at::kFloat && dim_t.numel() == 128 && unact.is_cuda() && dim_t.is_cuda(),
+              "two_stage_select: logits [B,S,C], unact [B,S,4], dim_t [128], fp32 CUDA");
+  TORCH_CHECK(unact.device() == logits.device() && dim_t.device() == logits.device(),
+              "two_stage_select: logits, unact and dim_t must be on one device");
+  const at::Tensor lg = logits.contiguous(), ua = unact.contiguous(), dt = dim_t.contiguous();
+  const int64_t B = lg.size(0), S = lg.size(1), C = lg.size(2);
+  const c10::cuda::CUDAGuard guard(logits.device());
+  auto fopt = lg.options();
+  at::Tensor keys = at::empty({B, S}, fopt.dtype(at::kInt));
+  at::Tensor index = at::empty({B, k}, fopt.dtype(at::kLong)), boxes = at::empty({B, k, 4}, fopt);
+  at::Tensor ref = at::empty({B, k, 4}, fopt), embed = at::empty({B, k, 512}, fopt);
+  const int rc = tfb200_two_stage_select_f32(lg.data_ptr<float>(), ua.data_ptr<float>(), dt.data_ptr<float>(),
+                                             reinterpret_cast<uint32_t*>(keys.data_ptr<int>()), index.data_ptr<int64_t>(),
+                                             boxes.data_ptr<float>(), ref.data_ptr<float>(), embed.data_ptr<float>(), int(B),
+                                             int(S), int(C), int(k), c10::cuda::getCurrentCUDAStream().stream());
+  TORCH_CHECK(rc == 0, "two_stage_select failed (code ", rc, ")");
+  return {index, boxes, ref, embed};
 }
 
 // ---- SetCriterion / matcher on the device (csrc/set_loss.cu) ------------------------------------------------------------
@@ -1609,6 +1723,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("add_dropout_layernorm_seeded_backward", &add_dropout_layernorm_seeded_backward);
   m.def("colsum", &colsum);
   m.def("lsa", &lsa);
+  m.def("lsa_wide", &lsa_wide);
+  m.def("two_stage_proposals", &two_stage_proposals);
+  m.def("two_stage_mask_rows", &two_stage_mask_rows);
+  m.def("two_stage_select", &two_stage_select);
   m.def("match_cost", &match_cost);
   m.def("set_loss_forward", &set_loss_forward);
   m.def("set_loss_backward", &set_loss_backward);

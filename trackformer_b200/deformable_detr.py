@@ -5,7 +5,8 @@ Mirror of ``DETR`` (src/trackformer/models/detr.py:17-128, the vanilla detector 
 ``DeformableDETR`` (src/trackformer/models/deformable_detr.py:29-283) with the same forward signature
 ``(samples, targets=None, prev_features=None) -> (out, targets, features_all, memory_per_level, hs)`` and the
 same parameter names (``input_proj.{l}.{0,1}``, ``class_embed.{k}``, ``bbox_embed.{k}.layers.{j}``,
-``query_embed``, ``transformer.*``, ``backbone.*``).  Two-stage and mask heads are outside the hot path.
+``query_embed``, ``transformer.*``, ``backbone.*``).  Two-stage (:92-113, 223-259) needs ``with_box_refine``: its
+``dec_layers + 1``-th class / box head scores the encoder proposals, reported as ``out["enc_outputs"]``.
 """
 from __future__ import annotations
 
@@ -132,15 +133,20 @@ class DeformableDETR(DETR):
     def __init__(self, backbone, transformer, num_classes, num_queries, num_feature_levels, aux_loss=True,
                  with_box_refine=False, two_stage=False, overflow_boxes=False, multi_frame_attention=False,
                  multi_frame_encoding=False, merge_frame_features=False):
+        if two_stage and not with_box_refine:
+            raise ValueError("two-stage Deformable DETR needs with_box_refine: its decoder refines the selected "
+                             "proposals with the per-layer box heads")
+        if two_stage and multi_frame_attention:
+            raise NotImplementedError("two-stage Deformable DETR with multi-frame attention: the proposal widths would "
+                                      "grow with a level index that runs over both frames' levels")
         super().__init__(backbone, transformer, num_classes, num_queries, aux_loss)
-        if two_stage:
-            raise NotImplementedError("two-stage Deformable-DETR is outside the hot path")
         self.merge_frame_features = merge_frame_features
         self.multi_frame_attention = multi_frame_attention
         self.multi_frame_encoding = multi_frame_encoding
         self.overflow_boxes = overflow_boxes
         self.num_feature_levels = num_feature_levels
-        self.query_embed = nn.Embedding(num_queries, self.hidden_dim * 2)    # (positional | content) halves
+        if not two_stage:       # two-stage keeps DETR's (unused) embedding: its queries come from the encoder
+            self.query_embed = nn.Embedding(num_queries, self.hidden_dim * 2)    # (positional | content) halves
 
         chans = backbone.num_channels[-3:]
         if num_feature_levels > 1:
@@ -169,7 +175,7 @@ class DeformableDETR(DETR):
             nn.init.xavier_uniform_(p[0].weight, gain=1)
             nn.init.zeros_(p[0].bias)
 
-        n_pred = transformer.decoder.num_layers
+        n_pred = transformer.decoder.num_layers + (1 if two_stage else 0)    # two-stage: + the encoder head
         if with_box_refine:
             self.class_embed = _clones(self.class_embed, n_pred)
             self.bbox_embed = _clones(self.bbox_embed, n_pred)
@@ -180,6 +186,10 @@ class DeformableDETR(DETR):
             self.class_embed = nn.ModuleList([self.class_embed for _ in range(n_pred)])
             self.bbox_embed = nn.ModuleList([self.bbox_embed for _ in range(n_pred)])
             self.transformer.decoder.bbox_embed = None
+        if two_stage:
+            self.transformer.decoder.class_embed = self.class_embed
+            for box_embed in self.bbox_embed:
+                nn.init.constant_(box_embed.layers[-1].bias.data[2:], 0.0)
         if self.merge_frame_features:
             self.merge_features = _clones(nn.Conv2d(self.hidden_dim * 2, self.hidden_dim, kernel_size=1),
                                           num_feature_levels)
@@ -226,11 +236,20 @@ class DeformableDETR(DETR):
         """(logits [layers, N, Q, classes], boxes [layers, N, Q, 4]) of the latest forward call, or None"""
         return self._call_scratch().value
 
+    @property
+    def encoder_heads(self):
+        """two-stage: (logits [N, S, classes], boxes [N, S, 4]) of the encoder head of the latest forward call -- the
+        tensors of ``out["enc_outputs"]`` -- or None"""
+        holder = self.__dict__.get("_enc_scratch")
+        return None if holder is None else holder.value
+
     def forward(self, samples: NestedTensor, targets: list = None, prev_features=None, prev_valid=None):
         """``prev_valid`` [B] bool (optional, with ``prev_features``): where False, image b has no previous frame and
         its own features stand in for ``prev_features`` -- as a whole call with ``prev_features=None`` does.  The select
         runs on the device, so a CUDA graph can take the flags as a static input."""
         self._call_scratch().value = None                # do not keep the previous call's graph alive
+        enc_scratch = self.__dict__.setdefault("_enc_scratch", _CallScratch())
+        enc_scratch.value = None
         if not isinstance(samples, NestedTensor):
             samples = nested_tensor_from_tensor_list(samples)
         features_all, pos = self.backbone(samples)
@@ -249,8 +268,8 @@ class DeformableDETR(DETR):
         for frame, frame_feat in enumerate(frames):
             self._project_levels(frame, frame_feat, prev_features, pos, src_list, mask_list, pos_list)
 
-        hs, memory, init_reference, inter_references, refined_boxes, _ = self.transformer(
-            src_list, mask_list, pos_list, self.query_embed.weight, targets)
+        hs, memory, init_reference, inter_references, refined_boxes, enc_outputs = self.transformer(
+            src_list, mask_list, pos_list, None if self.two_stage else self.query_embed.weight, targets)
 
         logits = torch.stack([self.class_embed[lvl](hs[lvl]) for lvl in range(hs.shape[0])])
         if refined_boxes is not None and self.with_box_refine and refined_boxes.shape[0] == hs.shape[0]:
@@ -268,6 +287,10 @@ class DeformableDETR(DETR):
         out = {"pred_logits": logits[-1], "pred_boxes": boxes[-1], "hs_embed": hs[-1]}
         if self.aux_loss:
             out["aux_outputs"] = self._set_aux_loss(logits, boxes)
+        if enc_outputs is not None:
+            enc_heads = (enc_outputs[0], enc_outputs[1].sigmoid())
+            enc_scratch.value = enc_heads
+            out["enc_outputs"] = {"pred_logits": enc_heads[0], "pred_boxes": enc_heads[1]}
 
         # encoder memory re-sliced to one NCHW map per level (consumed by the tracker / mask heads)
         bsz, _, ch = memory.shape

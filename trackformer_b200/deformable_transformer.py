@@ -9,18 +9,25 @@ config uses -- cfgs/train_deformable.yaml sets ``with_box_refine: true`` and lea
   track-query concatenation [prev hs_embed ; query tgt], zero query_pos for tracks    :202-225
   separate prev/current-frame encoder passes for multi-frame attention                :160-173
 
-Module and parameter names equal the reference's, so ``state_dict`` round-trips.  Two-stage proposal
-generation (:77-122,:180-194) is not on the hot path of any shipped configuration and is not built.
+  two-stage: encoder proposals, encoder head, top-k query selection and sine query embedding    :77-122,180-194
+
+Module and parameter names equal the reference's, so ``state_dict`` round-trips.  Two-stage runs on CUDA through
+csrc/two_stage.cu (one launch for the proposals and the masked memory, one for the selection, its embedding and the
+reference points) and on the CPU as the reference's torch ops; it does not take track queries or separate per-frame
+encoders (the detector classes refuse those combinations).
 """
 from __future__ import annotations
 
 import copy
-
+import math
 import os
 
 import torch
 import torch.nn.functional as F
 from torch import nn
+
+from torch.autograd import Function
+from torch.autograd.function import once_differentiable
 
 from . import seeds, small_attention
 from .fused_linear import ffn, ffn_fusable, linear as fused_linear, relu_dropout
@@ -46,6 +53,74 @@ def _add_pos(x, pos):
 
 # A/B switch (measurement only): True forces nn.MultiheadAttention's unfused bmm / softmax / bmm path
 _MHA_NEED_WEIGHTS = os.environ.get("TFB200_MHA_NEED_WEIGHTS", "0") == "1"
+
+
+def proposal_dim_t(device) -> torch.Tensor:
+    """The 128 frequencies of get_proposal_pos_embed (:93-95), computed by torch as the reference computes them."""
+    dim_t = torch.arange(128, dtype=torch.float32)
+    return (10000 ** (2 * (dim_t // 2) / 128)).to(device)
+
+
+def proposal_pos_embed(proposals: torch.Tensor) -> torch.Tensor:
+    """[N, L, 4] unactivated boxes -> [N, L, 512] sine embedding (deformable_transformer.py:89-102)."""
+    dim_t = proposal_dim_t(proposals.device)
+    proposals = proposals.sigmoid() * (2 * math.pi)
+    pos = proposals[:, :, :, None] / dim_t
+    return torch.stack((pos[:, :, :, 0::2].sin(), pos[:, :, :, 1::2].cos()), dim=4).flatten(2)
+
+
+def encoder_output_proposals(memory, padding_mask, hw):
+    """(masked memory, proposal logits [N, S, 4]) of gen_encoder_output_proposals (:104-133) without its encoder head;
+    ``padding_mask`` [N, S] (True = padded) or None for an unpadded batch.  The torch route (CPU, non-fp32)."""
+    n = memory.shape[0]
+    if padding_mask is None:
+        padding_mask = torch.zeros(memory.shape[:2], dtype=torch.bool, device=memory.device)
+    proposals, cur = [], 0
+    for lvl, (h, w) in enumerate(hw):
+        m = padding_mask[:, cur:cur + h * w].view(n, h, w, 1)
+        valid_h = torch.sum(~m[:, :, 0, 0], 1)
+        valid_w = torch.sum(~m[:, 0, :, 0], 1)
+        gy, gx = torch.meshgrid(torch.linspace(0, h - 1, h, dtype=torch.float32, device=memory.device),
+                                torch.linspace(0, w - 1, w, dtype=torch.float32, device=memory.device), indexing="ij")
+        grid = torch.cat([gx.unsqueeze(-1), gy.unsqueeze(-1)], -1)
+        scale = torch.cat([valid_w.unsqueeze(-1), valid_h.unsqueeze(-1)], 1).view(n, 1, 1, 2)
+        grid = (grid.unsqueeze(0).expand(n, -1, -1, -1) + 0.5) / scale
+        wh = torch.ones_like(grid) * 0.05 * (2.0 ** lvl)
+        proposals.append(torch.cat((grid, wh), -1).view(n, -1, 4))
+        cur += h * w
+    out = torch.cat(proposals, 1)
+    valid = ((out > 0.01) & (out < 0.99)).all(-1, keepdim=True)
+    out = torch.log(out / (1 - out))
+    out = out.masked_fill(padding_mask.unsqueeze(-1), float("inf")).masked_fill(~valid, float("inf"))
+    masked = memory.masked_fill(padding_mask.unsqueeze(-1), 0.0).masked_fill(~valid, 0.0)
+    return masked, out
+
+
+class _MaskedMemory(Function):
+    """memory -> (memory with the invalid proposal rows zeroed, proposal logits, valid flags) on CUDA: one launch of the
+    proposal kernel, or -- with ``memo`` = (proposal logits, flags) of an unpadded geometry -- of the row mask alone.
+    The gradient is masked the same way (one launch)."""
+
+    @staticmethod
+    def forward(ctx, memory, padding_mask, hw_flat, memo):
+        from . import ext
+        m = ext.load()
+        if memo is not None:
+            prop, valid = memo
+            masked = m.two_stage_mask_rows(memory, valid)
+        else:
+            prop, valid, masked = m.two_stage_proposals(padding_mask, memory, hw_flat, memory.shape[0],
+                                                        memory.device.index)
+        ctx.save_for_backward(valid)
+        ctx.mark_non_differentiable(prop, valid)
+        return masked, prop, valid
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_masked, _g_prop, _g_valid):
+        from . import ext
+        valid, = ctx.saved_tensors
+        return ext.load().two_stage_mask_rows(g_masked.contiguous(), valid), None, None, None
 
 
 class DeformableTransformerEncoderLayer(nn.Module):
@@ -214,8 +289,9 @@ class DeformableTransformer(nn.Module):
                  dec_n_points=4, enc_n_points=4, two_stage=False, two_stage_num_proposals=300,
                  multi_frame_attention_separate_encoder=False):
         super().__init__()
-        if two_stage:
-            raise NotImplementedError("two-stage Deformable-DETR is outside the hot path (no shipped config uses it)")
+        if two_stage and multi_frame_attention_separate_encoder:
+            raise NotImplementedError("two-stage Deformable DETR with multi-frame attention: the proposal widths would "
+                                      "grow over both frames' levels")
         self.d_model = d_model
         self.nhead = nhead
         self.two_stage = two_stage
@@ -231,8 +307,16 @@ class DeformableTransformer(nn.Module):
             DeformableTransformerDecoderLayer(d_model, dim_feedforward, dropout, activation, num_feature_levels,
                                               nhead, dec_n_points), num_decoder_layers, return_intermediate_dec)
         self.level_embed = nn.Parameter(torch.Tensor(num_feature_levels, d_model))
-        self.reference_points = nn.Linear(d_model, 2)
+        if two_stage:
+            self.enc_output = nn.Linear(d_model, d_model)
+            self.enc_output_norm = nn.LayerNorm(d_model)
+            self.pos_trans = nn.Linear(d_model * 2, d_model * 2)
+            self.pos_trans_norm = nn.LayerNorm(d_model * 2)
+        else:
+            self.reference_points = nn.Linear(d_model, 2)
+        self.selected_tokens = None         # two-stage: [N, k] token indices chosen by the latest forward
         self._shapes_memo = {}
+        self._proposal_memo = {}
         self._reset_parameters()
 
     def _reset_parameters(self):
@@ -242,8 +326,9 @@ class DeformableTransformer(nn.Module):
         for mod in self.modules():
             if isinstance(mod, MSDeformAttn):
                 mod._reset_parameters()
-        nn.init.xavier_uniform_(self.reference_points.weight, gain=1.0)
-        nn.init.zeros_(self.reference_points.bias)
+        if not self.two_stage:
+            nn.init.xavier_uniform_(self.reference_points.weight, gain=1.0)
+            nn.init.zeros_(self.reference_points.bias)
         nn.init.normal_(self.level_embed)
 
     def _shapes_tensor(self, hw, device):
@@ -277,8 +362,64 @@ class DeformableTransformer(nn.Module):
                 memo[key] = hit
         return hit
 
+    def _proposals(self, memory, enc_mask, hw):
+        """(masked memory, proposal logits) of the encoder output: the kernels on CUDA fp32, the reference's ops
+        elsewhere.  An unpadded batch's proposals depend on its geometry only and are made once."""
+        if not (memory.is_cuda and memory.dtype == torch.float32):
+            return encoder_output_proposals(memory, enc_mask, hw)
+        hw_flat = [v for pair in hw for v in pair]
+        memo = None
+        if enc_mask is None:
+            key = (tuple(hw), memory.shape[0], memory.device)
+            memo = self._proposal_memo.get(key)
+            if memo is None or torch.is_inference_mode_enabled():
+                from . import ext
+                # made on the memory's device, whichever device is current
+                prop, valid, _ = ext.load().two_stage_proposals(None, None, hw_flat, memory.shape[0],
+                                                                memory.device.index)
+                memo = (prop, valid)
+                if not torch.is_inference_mode_enabled():
+                    self._proposal_memo[key] = memo
+        masked, prop, _ = _MaskedMemory.apply(memory.contiguous(), enc_mask, hw_flat, memo)
+        return masked, prop
+
+    def _dim_t(self, device):
+        memo = self.__dict__.setdefault("_dim_t_memo", {})
+        t = memo.get(device)
+        if t is None or torch.is_inference_mode_enabled():
+            t = proposal_dim_t(device)
+            if not torch.is_inference_mode_enabled():
+                memo[device] = t
+        return t
+
+    def two_stage_queries(self, memory, enc_mask, hw):
+        """Encoder head, top-k selection and query embedding of deformable_transformer.py:180-194 ->
+        (query_pos, tgt, reference boxes [N, k, 4], encoder class logits [N, S, C], unactivated boxes [N, S, 4])."""
+        masked, proposals = self._proposals(memory, enc_mask, hw)
+        out_memory = self.enc_output_norm(fused_linear(masked, self.enc_output.weight, self.enc_output.bias))
+        last = self.decoder.num_layers
+        head = self.decoder.class_embed[last]
+        enc_class = fused_linear(out_memory, head.weight, head.bias)
+        enc_unact = self.decoder.bbox_embed[last](out_memory) + proposals
+        k = self.two_stage_num_proposals
+        if enc_class.is_cuda and enc_class.dtype == torch.float32:
+            from . import ext
+            idx, boxes, reference, embed = ext.load().two_stage_select(enc_class.detach(), enc_unact.detach(),
+                                                                      self._dim_t(enc_class.device), k)
+        else:
+            idx = torch.topk(enc_class[..., 0], k, dim=1)[1]
+            boxes = torch.gather(enc_unact, 1, idx.unsqueeze(-1).repeat(1, 1, 4)).detach()
+            reference = boxes.sigmoid()
+            embed = proposal_pos_embed(boxes)
+        self.selected_tokens = idx
+        pos_trans_out = self.pos_trans_norm(fused_linear(embed, self.pos_trans.weight, self.pos_trans.bias))
+        query_pos, tgt = torch.split(pos_trans_out, memory.shape[-1], dim=2)
+        return query_pos, tgt, reference, enc_class, enc_unact
+
     def forward(self, srcs, masks, pos_embeds, query_embed=None, targets=None):
-        assert query_embed is not None
+        """-> (hs, memory, init_reference, inter_references, refined boxes or None, encoder outputs): the last is None,
+        or with two-stage (class logits [N, S, C], unactivated boxes [N, S, 4]) of the encoder head."""
+        assert self.two_stage or query_embed is not None
         if self.training and srcs[0].is_cuda:
             seeds.begin_step(srcs[0].device)      # one launch draws the dropout seeds of every fused site of this pass
         hw, src_l, pos_l = [], [], []
@@ -310,13 +451,17 @@ class DeformableTransformer(nn.Module):
             memory = self.encoder(src_flat, spatial_shapes, valid_ratios, pos_flat, enc_mask)
 
         bs, _, c = memory.shape
-        query_pos, tgt = torch.split(query_embed, c, dim=1)
-        query_pos = query_pos.unsqueeze(0).expand(bs, -1, -1)
-        tgt = tgt.unsqueeze(0).expand(bs, -1, -1)
-        reference_points = self.reference_points(query_pos).sigmoid()
-        padded_queries = None
+        padded_queries = enc_outputs = None
+        if self.two_stage:
+            query_pos, tgt, reference_points, enc_class, enc_unact = self.two_stage_queries(memory, enc_mask, hw)
+            enc_outputs = (enc_class, enc_unact)
+        else:
+            query_pos, tgt = torch.split(query_embed, c, dim=1)
+            query_pos = query_pos.unsqueeze(0).expand(bs, -1, -1)
+            tgt = tgt.unsqueeze(0).expand(bs, -1, -1)
+            reference_points = self.reference_points(query_pos).sigmoid()
 
-        if targets is not None and "track_query_hs_embeds" in targets[0]:
+        if not self.two_stage and targets is not None and "track_query_hs_embeds" in targets[0]:
             # track queries: previous-frame output embeddings as content, zero positional part, previous box
             # centres as reference points; they are prepended to the object queries
             prev_hs = torch.stack([t["track_query_hs_embeds"] for t in targets])
@@ -333,7 +478,7 @@ class DeformableTransformer(nn.Module):
         hs, inter_references = self.decoder(tgt, reference_points, memory, spatial_shapes, valid_ratios,
                                             query_pos, enc_mask, None, padded_queries)
         refined, self.decoder.refined_boxes = self.decoder.refined_boxes, None     # (do not keep the graph alive)
-        return hs, memory, init_reference, inter_references, refined, None
+        return hs, memory, init_reference, inter_references, refined, enc_outputs
 
 
 def build_deforamble_transformer(args):

@@ -140,8 +140,14 @@ class DETRTrackingBase(nn.Module):
         return super().forward(samples, targets, prev_features, prev_valid)
 
 
+TWO_STAGE_TRACKING = ("two-stage Deformable DETR does not take track queries: its decoder queries are the selected "
+                      "encoder proposals, and the reference's two-stage branch skips the track-query concatenation")
+
+
 class DeformableDETRTracking(DETRTrackingBase, DeformableDETR):
     def __init__(self, tracking_kwargs, detr_kwargs):
+        if detr_kwargs.get("two_stage"):
+            raise NotImplementedError(TWO_STAGE_TRACKING)
         DeformableDETR.__init__(self, **detr_kwargs)
         DETRTrackingBase.__init__(self, **tracking_kwargs)
 

@@ -9,6 +9,9 @@ With ``masks=True`` it builds the segmentation models of src/trackformer/models/
 (``[Deformable]DETRSegm`` / ``[Deformable]DETRSegmTracking``) and adds the ``masks`` loss and the ``segm``
 post-processor (:42-45, 86-88, 103-104, 121-125); the panoptic post-processor is not provided.
 
+With ``two_stage=True`` (deformable, ``with_box_refine`` required) it builds two-stage Deformable DETR and adds the
+``_enc`` loss weights of the encoder proposals (:99-100).
+
 ``vanilla_args(...)`` gives cfgs/train.yaml alone (vanilla DETR), optionally with train_tracking.yaml.
 ``default_args(...)`` reproduces the values of cfgs/train.yaml overlaid with train_deformable.yaml and,
 optionally, train_tracking.yaml / train_multi_frame.yaml (the named sacred configs of src/train.py:24-35), so
@@ -94,6 +97,9 @@ def num_classes_for(dataset: str) -> int:
 def build_model(args):
     if args.masks and args.dataset == "coco_panoptic":
         raise NotImplementedError("the panoptic post-processor is not provided")
+    if args.two_stage and not (args.deformable and args.with_box_refine):
+        raise ValueError("two_stage needs the deformable model with with_box_refine: its decoder refines the selected "
+                         "encoder proposals with the per-layer box heads")
     num_classes = num_classes_for(args.dataset)
     backbone = build_backbone(args)
     matcher = build_matcher(args)
@@ -134,6 +140,8 @@ def build_model(args):
         base = dict(weight_dict)
         for i in range(args.dec_layers - 1):
             weight_dict.update({f"{k}_{i}": v for k, v in base.items()})
+        if args.two_stage:
+            weight_dict.update({f"{k}_enc": v for k, v in base.items()})
     criterion = SetCriterion(
         num_classes, matcher=matcher, weight_dict=weight_dict, eos_coef=args.eos_coef,
         losses=["labels", "boxes", "cardinality"] + (["masks"] if args.masks else []), focal_loss=args.focal_loss, focal_alpha=args.focal_alpha,

@@ -28,7 +28,7 @@ from torch.autograd.function import once_differentiable
 
 from . import ext
 from .deformable_detr import DETR, DeformableDETR
-from .detr_tracking import DETRTrackingBase
+from .detr_tracking import TWO_STAGE_TRACKING, DETRTrackingBase
 from .fused_linear import linear as fused_linear
 from .util import NestedTensor
 
@@ -415,6 +415,8 @@ class DeformableDETRSegm(DETRSegmBase, DeformableDETR):
 
 class DeformableDETRSegmTracking(DETRSegmBase, DETRTrackingBase, DeformableDETR):
     def __init__(self, mask_kwargs, tracking_kwargs, detr_kwargs):
+        if detr_kwargs.get("two_stage"):
+            raise NotImplementedError(TWO_STAGE_TRACKING)
         DeformableDETR.__init__(self, **detr_kwargs)
         DETRTrackingBase.__init__(self, **tracking_kwargs)
         DETRSegmBase.__init__(self, **mask_kwargs)

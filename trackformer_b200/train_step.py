@@ -36,7 +36,8 @@ from torch import nn
 
 
 class _DetectorCore(nn.Module):
-    """Tensor-in / tensors-out view of the detector for graph capture: frames -> (logits[K,B,Q,C], boxes[K,B,Q,4]).
+    """Tensor-in / tensors-out view of the detector for graph capture: frames -> (logits[K,B,Q,C], boxes[K,B,Q,4]), and
+    for a two-stage model the encoder head's (logits [B,S,C], boxes [B,S,4]) after them.
 
     With ``masks`` (segmentation models) the detector runs without its mask head and the mask branch's inputs
     follow the two heads: ``(logits, boxes, queries, memory, src, pad, fpn0, fpn1, fpn2)`` (``DETRSegmBase.mask_inputs``);
@@ -73,10 +74,14 @@ class _DetectorCore(nn.Module):
     def _heads(self, out):
         stacked = getattr(self.model, "stacked_heads", None)
         if stacked is not None and stacked[0].shape[0] == len(out["aux_outputs"]) + 1:
-            return tuple(stacked)                    # the very tensors the dictionary entries are slices of
-        logits = torch.stack([a["pred_logits"] for a in out["aux_outputs"]] + [out["pred_logits"]])
-        boxes = torch.stack([a["pred_boxes"] for a in out["aux_outputs"]] + [out["pred_boxes"]])
-        return logits, boxes
+            heads = tuple(stacked)                   # the very tensors the dictionary entries are slices of
+        else:
+            heads = (torch.stack([a["pred_logits"] for a in out["aux_outputs"]] + [out["pred_logits"]]),
+                     torch.stack([a["pred_boxes"] for a in out["aux_outputs"]] + [out["pred_boxes"]]))
+        enc = out.get("enc_outputs")
+        if enc is not None:
+            heads += (enc["pred_logits"], enc["pred_boxes"])
+        return heads
 
 
 class TrainStep:
@@ -100,6 +105,9 @@ class TrainStep:
         self._prev_plans, self._track_plans = {}, {}
         self.track_captures = 0
         segm = hasattr(model, "mask_head") or "masks" in getattr(criterion, "losses", ())
+        if masks and getattr(model, "two_stage", False):
+            raise NotImplementedError("TrainStep(masks=True) does not train two-stage segmentation models (its mask "
+                                      "step does not carry the encoder outputs); run the model and SetCriterion eagerly")
         if segm and not masks:
             raise NotImplementedError("TrainStep trains segmentation models only with masks=True (without it their "
                                       "mask losses would be dropped); or run the model and SetCriterion eagerly")
@@ -222,20 +230,19 @@ class TrainStep:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                      # warm-up off the capture path: cuDNN autotuning, memos
             for _ in range(3):
-                lg, bx = self.core(self.static_frames)
-                torch.autograd.backward((lg, bx), (torch.zeros_like(lg), torch.zeros_like(bx)))
+                heads = self.core(self.static_frames)
+                torch.autograd.backward(heads, [torch.zeros_like(h) for h in heads])
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         pool = self._pool = torch.cuda.graph_pool_handle()
         self.g_fwd = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.g_fwd, pool=pool):
-            self.s_logits, self.s_boxes = self.core(self.static_frames)
-        self.s_glogits = torch.zeros_like(self.s_logits)
-        self.s_gboxes = torch.zeros_like(self.s_boxes)
+            self.s_heads = self.core(self.static_frames)
+        self.s_gheads = [torch.zeros_like(h) for h in self.s_heads]     # cotangents, encoder heads last (two-stage)
         self.g_bwd = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.g_bwd, pool=pool):
             self.flat_grad.zero_()
-            torch.autograd.backward((self.s_logits, self.s_boxes), (self.s_glogits, self.s_gboxes))
+            torch.autograd.backward(self.s_heads, self.s_gheads)
         self.flat_grad.zero_()
 
     def _capture_masks(self, example: torch.Tensor) -> None:
@@ -266,8 +273,7 @@ class TrainStep:
                     self._phase_b()
                     self._phase_c()
                 else:
-                    lg, bx = self.core(self.static_frames)
-                    self._loss(lg, bx, self.s_targets, self.s_num_boxes).backward()
+                    self._heads_loss(self.core(self.static_frames), self.s_targets, self.s_num_boxes).backward()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         g = torch.cuda.CUDAGraph()
@@ -282,8 +288,7 @@ class TrainStep:
                 self._phase_c()
         else:
             with torch.cuda.graph(g, pool=self._pool):
-                lg, bx = self.core(self.static_frames)
-                loss = self._loss(lg, bx, self.s_targets, self.s_num_boxes)
+                loss = self._heads_loss(self.core(self.static_frames), self.s_targets, self.s_num_boxes)
                 self._backward_into_flat(loss)
                 self.s_loss = loss.detach()
         self.g_full = g
@@ -319,10 +324,10 @@ class TrainStep:
             return leaf
         self._trunk.cut = cut
         try:
-            logits, boxes = self.core(frames)
+            heads = self.core(frames)
         finally:
             self._trunk.cut = None
-        loss = self._loss(logits, boxes, targets, num_boxes)
+        loss = self._heads_loss(heads, targets, num_boxes)
         head = self.params[:self._i_bb]
         tags = list(rec)
         grads = torch.autograd.grad(loss, head + [rec[t][1] for t in tags], allow_unused=True)
@@ -406,11 +411,17 @@ class TrainStep:
             if g is None:
                 v.zero_()
 
-    def _loss(self, logits, boxes, targets, num_boxes=None, track_queries=False, with_dict=False):
+    def _heads_loss(self, heads, targets, num_boxes=None):
+        """``_loss`` of the detector's ``heads`` (see ``_DetectorCore``): two-stage encoder heads included"""
+        return self._loss(heads[0], heads[1], targets, num_boxes, enc=tuple(heads[2:4]) if len(heads) > 2 else None)
+
+    def _loss(self, logits, boxes, targets, num_boxes=None, track_queries=False, with_dict=False, enc=None):
         """Weighted total of the criterion's entries (engine.py:139-140: sum(loss_dict[k] * weight_dict[k]));
-        ``with_dict``: -> (total, loss dictionary)."""
+        ``with_dict``: -> (total, loss dictionary); ``enc``: a two-stage model's encoder (logits, boxes)."""
         if track_queries:
             loss_dict = self.criterion.forward_stacked(logits, boxes, targets, num_boxes, track_queries=True)
+        elif enc is not None:
+            loss_dict = self.criterion.forward_stacked(logits, boxes, targets, num_boxes, enc_outputs=enc)
         else:
             loss_dict = self.criterion.forward_stacked(logits, boxes, targets, num_boxes)
         total = self._total(loss_dict)
@@ -429,7 +440,9 @@ class TrainStep:
                 rows = [[float(wd.get(f"{n}_{i}", 0.0)) for i in range(k - 1)] + [float(wd.get(n, 0.0))] for n in names]
                 self._loss_w = torch.tensor(rows, dtype=stacked[0].dtype, device=stacked[0].device)
                 self._loss_w_key = key
-            return (torch.stack(stacked) * self._loss_w).sum()
+            total = (torch.stack(stacked) * self._loss_w).sum()
+            enc = [loss_dict[k] * wd[k] for k in loss_dict if k.endswith("_enc") and k in wd]     # two-stage encoder
+            return total + sum(enc) if enc else total
         return sum(loss_dict[k] * wd[k] for k in loss_dict if k in wd)
 
     # ------------------------------------------------------------------------------------------ masks
@@ -779,16 +792,13 @@ class TrainStep:
                 self._release_staging(dev)
                 staged = False
             self.g_fwd.replay()
-            logits = self.s_logits.detach().requires_grad_(True)
-            boxes = self.s_boxes.detach().requires_grad_(True)
-            loss = self._loss(logits, boxes, targets, num_boxes)
-            g_logits, g_boxes = torch.autograd.grad(loss, (logits, boxes))
-            self.s_glogits.copy_(g_logits)
-            self.s_gboxes.copy_(g_boxes)
+            heads = [h.detach().requires_grad_(True) for h in self.s_heads]
+            loss = self._heads_loss(heads, targets, num_boxes)
+            for dst, g in zip(self.s_gheads, torch.autograd.grad(loss, heads)):
+                dst.copy_(g)
             self.g_bwd.replay()
         else:
-            logits, boxes = self.core(frames)
-            loss = self._loss(logits, boxes, targets, num_boxes)
+            loss = self._heads_loss(self.core(frames), targets, num_boxes)
             self._backward_into_flat(loss)
         if self.world > 1:
             if self.phased:
