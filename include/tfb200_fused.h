@@ -590,6 +590,40 @@ int tfb200_frame_ingest_u8_f32(const uint8_t* src, int64_t src_row_stride, int H
                                const float* lut, float* dst, int64_t dst_row_stride, int64_t dst_plane_stride, int h,
                                int w, void* stream);
 
+/* Panoptic post-processing and PQ (csrc/panoptic.cu, routines in csrc/panoptic_core.h; reference: PostProcessPanoptic,
+ * models/detr_segmentation.py:256-388, and panopticapi's pq_compute).  All entries enqueue on `stream` and read
+ * nothing back; the per-image tables (int64 rows, layouts in panoptic_core.h) are built by the host.
+ * tfb200_panoptic_classes_f32: logits [B][Q][C] -> per row the first class of maximal fp32 softmax (cls), its
+ *   probability (score) and keep = cls != C - 1 && score > threshold.
+ * tfb200_panoptic_label_f32: one round of the label pass over the images flagged active in img [B][14]: masks
+ *   [B][Q][h][w] stride-4 logits bilinearly sampled at the processed size, the first surviving kept query of maximal
+ *   softmax per pixel (its stuff representative on a dedup pass) into map, and each label's target-size area (the
+ *   pixel weighted by the Pillow nearest-resize row and column counts) added to area (zeroed by the caller).
+ * tfb200_panoptic_final_f32: target-size maps (survivor position of the nearest source, 0 without survivors).
+ * tfb200_pq_update: per image of img [B][10] the intersection counts of the raw-id maps (cells zeroed here) and the
+ *   per-(image, category) tp / fp / fn / IoU sum and error records (err rows preset to {LLONG_MAX, LLONG_MAX, 0}).
+ * tfb200_pq_reduce: out [Kc][4] = sums over the records rows[0 .. n) in that order; err_out[0] the first i whose
+ *   record holds an error, or n.
+ * Limits: K <= TFB200_PANOPTIC_MAX_KEPT kept queries, G, P <= TFB200_PANOPTIC_MAX_SEGMENTS listed segments per image
+ * and side, Kc <= TFB200_PANOPTIC_MAX_CATEGORIES, pixels per image < 2^31, blocks >= ceil(pixels / 4096) of the
+ * largest image (the caller passes it).  Out of range: TFB200_E_SHAPE, and nothing is launched.                    */
+#define TFB200_PANOPTIC_MAX_KEPT 1024
+#define TFB200_PANOPTIC_MAX_SEGMENTS 1024
+#define TFB200_PANOPTIC_MAX_CATEGORIES 4096
+int tfb200_panoptic_classes_f32(const float* logits, int B, int Q, int C, float threshold, int32_t* cls, float* score,
+                                uint8_t* keep, void* stream);
+int tfb200_panoptic_label_f32(const float* masks, int B, int Q, int h, int w, const int64_t* img, int max_kept,
+                              const int32_t* kept_q, const int32_t* kept_alive, const int32_t* kept_rep,
+                              const int32_t* idx, int32_t* map, unsigned long long* area, int blocks, void* stream);
+int tfb200_panoptic_final_f32(const int64_t* img, int B, const int32_t* kept_alive, const int32_t* kept_pos,
+                              const int32_t* idx, const int32_t* map, int32_t* out, int blocks, void* stream);
+int tfb200_pq_update(const int64_t* img, int B, int Kc, int max_seg, const int32_t* maps, const int32_t* gt_id,
+                     const int32_t* gt_cat, const int32_t* gt_crowd, const double* gt_area, const int32_t* gt_json,
+                     const int32_t* pred_id, const int32_t* pred_cat, int* cells, int64_t n_cells, int64_t* pred_area,
+                     int32_t* stat_i, double* stat_iou, long long* err, int blocks, void* stream);
+int tfb200_pq_reduce(const int32_t* stat_i, const double* stat_iou, const long long* err, const int64_t* rows,
+                     int64_t n, int Kc, double* out, int64_t* err_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -18,6 +18,7 @@
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
+#include "interp_index.h"
 #include "launch_counter.h"
 
 namespace {
@@ -343,13 +344,7 @@ __global__ void sum_queries_kernel(const float* __restrict__ in, float* __restri
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// nearest source index of F.interpolate(mode="nearest") (aten/src/ATen/native/UpSample.h nearest_idx)
-__device__ __forceinline__ int nearest_src(int o, int in, int out) {
-  if (in == out) return o;
-  if (out == 2 * in) return o >> 1;
-  const float scale = float(in) / float(out);
-  return min(int(floorf(float(o) * scale)), in - 1);
-}
+using tfb200_interp::nearest_src;
 
 template <class Rows>
 __global__ void upsample_add_fwd_kernel(const float* __restrict__ x, const float* __restrict__ a,

@@ -24,6 +24,7 @@
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
+#include "interp_index.h"
 #include "launch_counter.h"
 
 namespace {
@@ -37,29 +38,9 @@ constexpr int kStageFloats = 8192;         // 32 KB of staged logits per pass
 constexpr int kMaxSmem = 200 * 1024;
 constexpr int kMaxBatch = 16;             // images per launch
 
-struct Lin {
-  int i0, i1;
-  float l0, l1;
-};
-
-// ATen nearest_idx (UpSample.h) for input size `in`, output size `out`
-__device__ __forceinline__ int nearest_src(int o, int in, int out) {
-  if (out == in) return o;
-  if (out == 2 * in) return o >> 1;
-  const float scale = float(in) / float(out);
-  return min(int(floorf(__fmul_rn(float(o), scale))), in - 1);
-}
-
-// ATen compute_source_index_and_lambda, linear mode, align_corners=False
-__device__ __forceinline__ Lin linear_src(int o, int in, int out) {
-  if (out == in) return {o, o, 1.f, 0.f};
-  const float scale = float(in) / float(out);
-  float s = __fsub_rn(__fmul_rn(scale, __fadd_rn(float(o), 0.5f)), 0.5f);
-  s = s < 0.f ? 0.f : s;
-  const int i0 = min(int(floorf(s)), in - 1);
-  const float l1 = fminf(fmaxf(__fsub_rn(s, float(i0)), 0.f), 1.f);
-  return {i0, i0 + (i0 < in - 1 ? 1 : 0), __fsub_rn(1.f, l1), l1};
-}
+using tfb200_interp::Lin;
+using tfb200_interp::linear_src;
+using tfb200_interp::nearest_src;
 
 __device__ __forceinline__ unsigned slot_of(int id, int mask) {
   unsigned x = unsigned(id);

@@ -7,7 +7,8 @@ postprocessors)`` with the same class counts (:17-26), model classes (:48-83: ``
 
 With ``masks=True`` it builds the segmentation models of src/trackformer/models/detr_segmentation.py
 (``[Deformable]DETRSegm`` / ``[Deformable]DETRSegmTracking``) and adds the ``masks`` loss and the ``segm``
-post-processor (:42-45, 86-88, 103-104, 121-125); the panoptic post-processor is not provided.
+post-processor (:42-45, 86-88, 103-104, 121-125); with ``dataset="coco_panoptic"`` (250 classes, softmax head only) also
+the ``panoptic`` post-processor (:124-128).
 
 With ``two_stage=True`` (deformable, ``with_box_refine`` required) it builds two-stage Deformable DETR and adds the
 ``_enc`` loss weights of the encoder proposals (:99-100).
@@ -30,7 +31,8 @@ from .deformable_detr import DETR, DeformableDETR, DeformablePostProcess, PostPr
 from .deformable_transformer import build_deforamble_transformer
 from .detr_tracking import DeformableDETRTracking, DETRTracking
 from .matcher import build_matcher
-from .segmentation import DeformableDETRSegm, DeformableDETRSegmTracking, DETRSegm, DETRSegmTracking, PostProcessSegm
+from .segmentation import (PANOPTIC_SIGMOID, DeformableDETRSegm, DeformableDETRSegmTracking, DETRSegm, DETRSegmTracking,
+                           PostProcessPanoptic, PostProcessSegm)
 from .transformer import build_transformer
 
 _TRAIN_YAML = dict(   # cfgs/train.yaml (model / loss keys only)
@@ -95,8 +97,8 @@ def num_classes_for(dataset: str) -> int:
 
 
 def build_model(args):
-    if args.masks and args.dataset == "coco_panoptic":
-        raise NotImplementedError("the panoptic post-processor is not provided")
+    if args.masks and args.dataset == "coco_panoptic" and args.focal_loss:
+        raise NotImplementedError(PANOPTIC_SIGMOID)
     if args.two_stage and not (args.deformable and args.with_box_refine):
         raise ValueError("two_stage needs the deformable model with with_box_refine: its decoder refines the selected "
                          "encoder proposals with the per-layer box heads")
@@ -151,4 +153,7 @@ def build_model(args):
     postprocessors = {"bbox": DeformablePostProcess() if args.focal_loss else PostProcess()}
     if args.masks:
         postprocessors["segm"] = PostProcessSegm()
+        if args.dataset == "coco_panoptic":
+            is_thing_map = {i: i <= 90 for i in range(201)}
+            postprocessors["panoptic"] = PostProcessPanoptic(is_thing_map, threshold=0.85)
     return model, criterion, postprocessors

@@ -523,3 +523,165 @@ class PostProcessSegm(nn.Module):
                 masks = masks[results_mask[i]]
             results[i]["masks"] = masks
         return results
+
+
+def pillow_nearest_src(n_in: int, n_out: int) -> np.ndarray:
+    """Source index of each of `n_out` outputs of Pillow's NEAREST resize from `n_in`: int(v), v = s / 2 then v += s
+    accumulated in double, s = n_in / n_out (ImagingScaleAffine).  Not ATen's nearest index."""
+    s = n_in / n_out
+    steps = np.full(n_out, s, np.float64)
+    steps[0] = s / 2
+    return np.add.accumulate(steps).astype(np.int64)
+
+
+PANOPTIC_SIGMOID = ("panoptic post-processing needs a softmax classifier: PostProcessPanoptic takes a softmax over the "
+                    "class logits and treats the last column as 'no object', so on a sigmoid (focal-loss) head it would "
+                    "silently drop the last real class")
+
+
+class PostProcessPanoptic(nn.Module):
+    """The model's outputs as COCO panoptic results (detr_segmentation.py:256-388): one dict per image,
+    ``{"png_string": bytes, "segments_info": [{"id", "isthing", "category_id", "area"}]}``.
+
+    The reference's semantics, quirks included: kept queries are ``argmax != last and max softmax > threshold``; their
+    padded stride-4 logits are bilinearly upsampled straight to the unpadded processed size; every pixel takes the
+    first kept query of maximal softmax; on the first pass the later queries of a stuff class merge into its first; the
+    map is resized to the target size with Pillow's NEAREST; while any segment has an area <= 4 pixels at target size
+    those segments are dropped and the map is recomputed from the survivors (without the merge).  Segment ids are the
+    survivors' positions.  A kept class missing from ``is_thing_map`` raises KeyError.
+
+    CUDA fp32 only (csrc/panoptic.cu): one class launch, then rounds of one label launch over the whole batch with one
+    read-back of the areas per round, and one launch writing the int32 target-size maps; the PNG is encoded on the
+    host.  ``maps_on_device=True`` adds each image's map as ``"label_map"`` (int32 [H, W] on the model's device), which
+    ``PanopticEvaluator.update`` scores without decoding the PNG."""
+
+    def __init__(self, is_thing_map, threshold=0.85, maps_on_device=False):
+        super().__init__()
+        self.threshold = threshold
+        self.is_thing_map = is_thing_map
+        self.maps_on_device = maps_on_device
+
+    @torch.no_grad()
+    def forward(self, outputs, processed_sizes, target_sizes=None):
+        from .panoptic_eval import png_of
+        maps, infos = self.label_maps(outputs, processed_sizes, target_sizes)
+        host = [m.cpu().numpy() for m in maps]
+        preds = []
+        for m, d, info in zip(host, maps, infos):
+            pred = {"png_string": png_of(m), "segments_info": info}
+            if self.maps_on_device:
+                pred["label_map"] = d
+            preds.append(pred)
+        return preds
+
+    @torch.no_grad()
+    def label_maps(self, outputs, processed_sizes, target_sizes=None, lib=None):
+        """The target-size id maps (int32 [H, W] on the outputs' device) and each image's ``segments_info``: what
+        ``forward`` returns before the PNG encode.  ``lib``: a ctypes library with the C entries of csrc/panoptic.cu
+        (default: the package's) -- the tests pass a host build of the same routines and CPU tensors."""
+        from .panoptic_eval import MAX_KEPT, BLOCK_PIXELS, _library, check, stream_of
+        if target_sizes is None:
+            target_sizes = processed_sizes
+        assert len(processed_sizes) == len(target_sizes)
+        logits, masks = outputs["pred_logits"], outputs["pred_masks"]
+        assert len(logits) == len(masks) == len(target_sizes)
+        if lib is None and not (logits.is_cuda and masks.is_cuda):
+            raise NotImplementedError("PostProcessPanoptic runs on CUDA outputs (csrc/panoptic.cu)")
+        dev = logits.device
+        lib, stream = lib or _library(), stream_of(dev)
+        B, Q, C = logits.shape
+        h, w = masks.shape[-2:]
+        logits = logits.float().contiguous()
+        masks = masks.float().reshape(B, Q, h, w).contiguous()
+        to_hw = lambda s: tuple(int(v) for v in (s.tolist() if torch.is_tensor(s) else s))
+        sizes = [to_hw(s) for s in processed_sizes]
+        tsizes = [to_hw(s) for s in target_sizes]
+
+        cls = torch.empty(B * Q, dtype=torch.int32, device=dev)
+        score = torch.empty(B * Q, dtype=torch.float32, device=dev)
+        keep = torch.empty(B * Q, dtype=torch.uint8, device=dev)
+        check(lib.tfb200_panoptic_classes_f32(logits.data_ptr(), B, Q, C, float(self.threshold), cls.data_ptr(),
+                                              score.data_ptr(), keep.data_ptr(), stream), "panoptic classes")
+        cls_h = cls.view(B, Q).cpu().numpy()
+        keep_h = keep.view(B, Q).cpu().numpy().astype(bool)
+
+        kept_q, kept_cls, rep, off = [], [], [], [0]
+        for b in range(B):
+            q = np.nonzero(keep_h[b])[0]
+            if len(q) > MAX_KEPT:
+                raise ValueError(f"PostProcessPanoptic: image {b} keeps {len(q)} queries, over the limit of {MAX_KEPT}")
+            c = cls_h[b, q]
+            first_of = {}
+            r = np.arange(len(q), dtype=np.int32)
+            for k, lab in enumerate(c.tolist()):
+                if not self.is_thing_map[lab]:                   # KeyError for an unknown class, as the reference
+                    r[k] = first_of.setdefault(lab, k)
+            kept_q.append(q.astype(np.int32))
+            kept_cls.append(c)
+            rep.append(r)
+            off.append(off[-1] + len(q))
+        n_kept = off[-1]
+        max_k = max((len(q) for q in kept_q), default=0)
+
+        # per-image geometry: Pillow's row / column sources and the processed rows / columns' mapped counts
+        idx, img = [], np.zeros((B, 14), np.int64)
+        io_ = mo = oo = 0
+        for b in range(B):
+            (H, W), (Ht, Wt) = sizes[b], tsizes[b]
+            rows, cols = pillow_nearest_src(H, Ht), pillow_nearest_src(W, Wt)
+            parts = [rows, cols, np.bincount(rows, minlength=H), np.bincount(cols, minlength=W)]
+            offs = []
+            for a in parts:
+                offs.append(io_)
+                idx.append(a.astype(np.int32))
+                io_ += len(a)
+            img[b] = (H, W, Ht, Wt, off[b], len(kept_q[b]), mo, offs[0], offs[1], offs[2], offs[3], oo,
+                      int(len(kept_q[b]) > 0), 1)
+            mo += H * W
+            oo += Ht * Wt
+        cat = lambda xs: np.concatenate(xs).astype(np.int32) if xs and sum(map(len, xs)) else np.zeros(1, np.int32)
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev, non_blocking=True)
+        idx_d = up(cat(idx))
+        kq_d, rep_d = up(cat(kept_q)), up(cat(rep))
+        label = torch.empty(max(mo, 1), dtype=torch.int32, device=dev)
+        area = torch.empty(max(n_kept, 1), dtype=torch.int64, device=dev)
+        alive = np.ones(max(n_kept, 1), np.int32)
+        blocks = max(1, max((H * W + BLOCK_PIXELS - 1) // BLOCK_PIXELS for H, W in sizes))
+        areas = np.zeros(n_kept, np.int64)
+        while img[:, 12].any():                                  # rounds over the whole batch
+            img_d, alive_d = up(img), up(alive)
+            area.zero_()
+            check(lib.tfb200_panoptic_label_f32(masks.data_ptr(), B, Q, h, w, img_d.data_ptr(), max_k,
+                                                kq_d.data_ptr(), alive_d.data_ptr(), rep_d.data_ptr(),
+                                                idx_d.data_ptr(), label.data_ptr(), area.data_ptr(), blocks, stream),
+                  "panoptic label")
+            got = area[:n_kept].cpu().numpy()                   # the round's one read-back
+            for b in range(B):
+                if not img[b, 12]:
+                    continue
+                s = slice(off[b], off[b + 1])
+                areas[s] = got[s]
+                small = (alive[s] == 1) & (got[s] <= 4)
+                img[b, 13] = 0                                   # later passes do not merge stuff duplicates
+                if small.any():
+                    alive[s][small] = 0
+                    img[b, 12] = int(alive[s].any())
+                else:
+                    img[b, 12] = 0
+        pos = np.zeros(max(n_kept, 1), np.int32)
+        infos = []
+        for b in range(B):
+            s = slice(off[b], off[b + 1])
+            surv = np.nonzero(alive[s] == 1)[0]
+            pos[off[b] + surv] = np.arange(len(surv), dtype=np.int32)
+            infos.append([{"id": i, "isthing": self.is_thing_map[int(kept_cls[b][k])],
+                           "category_id": int(kept_cls[b][k]), "area": int(areas[off[b] + k])}
+                          for i, k in enumerate(surv.tolist())])
+        out = torch.empty(max(oo, 1), dtype=torch.int32, device=dev)
+        img_d = up(img)
+        check(lib.tfb200_panoptic_final_f32(img_d.data_ptr(), B, up(alive).data_ptr(), up(pos).data_ptr(),
+                                            idx_d.data_ptr(), label.data_ptr(), out.data_ptr(),
+                                            max(1, max((Ht * Wt + BLOCK_PIXELS - 1) // BLOCK_PIXELS
+                                                       for Ht, Wt in tsizes)), stream), "panoptic final")
+        maps = [out[int(img[b, 11]):int(img[b, 11]) + Ht * Wt].view(Ht, Wt) for b, (Ht, Wt) in enumerate(tsizes)]
+        return maps, infos
