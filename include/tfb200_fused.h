@@ -624,6 +624,47 @@ int tfb200_pq_update(const int64_t* img, int B, int Kc, int max_seg, const int32
 int tfb200_pq_reduce(const int32_t* stat_i, const double* stat_iou, const long long* err, const int64_t* rows,
                      int64_t n, int Kc, double* out, int64_t* err_out, void* stream);
 
+/* COCO polygon segmentations as mask runs (csrc/coco_poly.cu, routines in csrc/coco_poly_core.h): pycocotools 2.0's
+ * rleFrPoly of every part, bit for bit, and the union of each annotation's parts (maskUtils.merge).  n_ann
+ * annotations, each of parts ann_part[a] .. ann_part[a + 1] (int64 [n_ann + 1]) and size ann_hw [n_ann][2] int32 h, w
+ * (h x w < 2^31); part p has vertices part_off[p] .. part_off[p + 1] (int64 [n_parts + 1], n_edges = the total < 2^31)
+ * of xy [n_edges][2] fp64 and annotation part_ann[p].  A box is given as its 4-vertex polygon.
+ * tfb200_coco_poly_count: sizes [5] int64 = {boundary points, toggles, status, first annotation of status bit 1,
+ *   first of bit 2 (n_ann when unset)}; status bit 1: a non-finite coordinate, bit 2: |5 c + .5| >= 2^31, bit 4: over
+ *   2^31 - 1 boundary points (toggles are then not counted).  ann_points [n_ann] int64: each annotation's points;
+ *   toggle_off [n_edges + 1] int32: the edges' toggle offsets, kept for tfb200_coco_poly_runs.
+ * tfb200_coco_poly_runs (after a count with status 0; n_toggles = sizes[1]): run_off [n_ann + 1] int64 and runs
+ *   [][2] uint32 (column-major start, length of each run of ones of the union; capacity n_toggles rows).
+ * tfb200_coco_rle_runs: n compressed COCO counts strings (chars[str_off[k] .. str_off[k + 1])) of h x w masks into
+ *   runs at run_cap_off[k] .. (caller's bound: floor(length / 2) per string); bounds [n][2] int64 = {begin, end};
+ *   a malformed string (or counts not summing to h x w) atomically mins its index into *first_bad (set by the
+ *   caller).
+ * tfb200_coco_masks_u8: out [N][H][W] uint8 from the runs of src[i] >= 0 (poly annotation, run_off / runs) or
+ *   src[i] < 0 (string -1 - src[i], rle_bounds / rle_runs).
+ * Workspaces: the *_workspace_bytes queries (0 for bad sizes), 256-byte aligned; about 8 B per edge for the count and
+ * 16 B per toggle plus CUB's segmented-sort buffers for the runs.  Sizes out of range: TFB200_E_SHAPE.              */
+#define TFB200_POLY_SIZES 5
+#define TFB200_POLY_SIZE_POINTS 0
+#define TFB200_POLY_SIZE_TOGGLES 1
+#define TFB200_POLY_SIZE_STATUS 2
+#define TFB200_POLY_SIZE_BAD_FINITE 3
+#define TFB200_POLY_SIZE_BAD_RANGE 4
+size_t tfb200_coco_poly_count_workspace_bytes(int n_parts, int n_ann, int64_t n_edges);
+int tfb200_coco_poly_count(const double* xy, const int64_t* part_off, const int32_t* part_ann,
+                           const int64_t* ann_part, const int32_t* ann_hw, int n_parts, int n_ann, int64_t n_edges,
+                           void* workspace, size_t workspace_bytes, int32_t* toggle_off, int64_t* ann_points,
+                           int64_t* sizes, void* stream);
+size_t tfb200_coco_poly_runs_workspace_bytes(int n_parts, int n_ann, int64_t n_toggles);
+int tfb200_coco_poly_runs(const double* xy, const int64_t* part_off, const int32_t* part_ann, const int64_t* ann_part,
+                          const int32_t* ann_hw, int n_parts, int n_ann, int64_t n_edges, const int32_t* toggle_off,
+                          int64_t n_toggles, void* workspace, size_t workspace_bytes, int64_t* run_off,
+                          uint32_t* runs, void* stream);
+int tfb200_coco_rle_runs(const uint8_t* chars, const int64_t* str_off, const int64_t* run_cap_off, int n, int h, int w,
+                         int64_t* bounds, uint32_t* runs, int64_t* first_bad, void* stream);
+int tfb200_coco_masks_u8(const int32_t* src, int N, int H, int W, const int64_t* poly_run_off,
+                         const uint32_t* poly_runs, const int64_t* rle_bounds, const uint32_t* rle_runs, uint8_t* out,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,8 +12,12 @@ sets `stats` on the host.
 
 The numbers are those of pycocotools 2.0's `COCOeval` with its default parameters, as the reference calls it,
 including its quirks: an annotation's own `ignore` key is replaced by `iscrowd`, and a detection matched to an
-annotation with id 0 is not a true positive.  Polygon ground-truth masks are not supported, and neither are
-keypoints.  pycocotools' per-image `evalImgs` dicts are not built.  CUDA only: there is no host fallback.
+annotation with id 0 is not a true positive.  Ground-truth masks may be RLEs (compressed or not) or polygon and
+box lists, which `COCO.annToRLE` rasterises: `CocoEvaluator` packs every polygon of the segm ground truth once and
+rasterises them in one call on its device (trackformer_b200.coco_masks, csrc/coco_poly.cu), bit for bit as
+pycocotools' `frPyObjects` + `merge`; an annotation's `area` still comes from the JSON.  `GroundTruth(dataset, True)`
+without a device rejects polygons.  Keypoints are not supported, and pycocotools' per-image `evalImgs` dicts are not
+built.  CUDA only: there is no host fallback.
 """
 from __future__ import annotations
 
@@ -26,7 +30,7 @@ import os
 import numpy as np
 import torch
 
-from . import mots
+from . import coco_masks, mots
 
 __all__ = ["CocoEvaluator", "Params", "GroundTruth", "kept_images", "MAX_DETS_PER_IMAGE", "MAX_GT_PER_IMAGE_CATEGORY"]
 
@@ -128,9 +132,11 @@ class GroundTruth:
 
     Rows are the annotations of each image in JSON order, stably sorted by category index within the image;
     `off[i] .. off[i + 1]` are image i's rows, images in the order of `dataset["images"]`.  Annotations of categories
-    outside `cat_ids` are left out, as pycocotools' `getAnnIds(catIds=...)` leaves them out."""
+    outside `cat_ids` are left out, as pycocotools' `getAnnIds(catIds=...)` leaves them out.  With `device`, the segm
+    ground truth's polygon and box-list segmentations are rasterised in one call there and read back once; without
+    it they raise NotImplementedError."""
 
-    def __init__(self, dataset: dict, segm: bool):
+    def __init__(self, dataset: dict, segm: bool, device=None):
         images = dataset.get("images", [])
         self.img_ids = np.asarray([int(im["id"]) for im in images], np.int64)
         self.row_of = {int(i): r for r, i in enumerate(self.img_ids)}
@@ -181,11 +187,24 @@ class GroundTruth:
             self.px = np.zeros(n, np.int64)
             runs = []
             self.run_off = np.zeros(n + 1, np.int64)
+            poly = {}
+            if device is not None:
+                rows_p = [i for i, (_, _, a) in enumerate(rows) if isinstance(a.get("segmentation"), list)]
+                for i in rows_p:
+                    r = rows[i][0]
+                    if int(self.height[r]) * int(self.width[r]) >= 2 ** 31:
+                        raise ValueError(f"coco_eval: image {self.img_ids[r]} is over 2^31 pixels")
+                if rows_p:
+                    p_off, p_runs = coco_masks.poly_runs(
+                        [rows[i][2]["segmentation"] for i in rows_p],
+                        [(int(self.height[rows[i][0]]), int(self.width[rows[i][0]])) for i in rows_p],
+                        [f"annotation {rows[i][2].get('id')}" for i in rows_p], device)
+                    poly = {i: p_runs[p_off[j]:p_off[j + 1]] for j, i in enumerate(rows_p)}
             for i, (r, _, a) in enumerate(rows):
                 h, w = int(self.height[r]), int(self.width[r])
                 if h * w >= 2 ** 31:
                     raise ValueError(f"coco_eval: image {self.img_ids[r]} is over 2^31 pixels")
-                ru = _runs(a, h, w)
+                ru = poly[i] if i in poly else _runs(a, h, w)
                 runs.append(ru)
                 self.run_off[i + 1] = self.run_off[i] + len(ru)
                 self.px[i] = int(ru[:, 1].sum()) if len(ru) else 0
@@ -395,7 +414,7 @@ class CocoEvaluator:
         self.coco_gt = coco_gt
         self.iou_types = tuple(iou_types)
         dataset = load_dataset(coco_gt)
-        self.gt = {t: GroundTruth(dataset, t == "segm") for t in self.iou_types}
+        self.gt = {t: GroundTruth(dataset, t == "segm", self.device if t == "segm" else None) for t in self.iou_types}
         self.coco_eval = {t: COCOevalGPU(t, self.gt[t].cat_ids.tolist()) for t in self.iou_types}
         self.img_ids = []
         self._records = {t: [] for t in self.iou_types}
