@@ -6,16 +6,13 @@ that sequence's detector's answer, laid out as `GraphedDetector.batched` lays it
 end of the kb padded slots, then the object queries).  So a MultiSequenceTracker over a Mux and one tracker per
 sequence over that sequence's own detector see the same detections, and any difference is the bookkeeping's.
 """
-import ctypes
-import os
-import subprocess
 
 import numpy as np
 import torch
 
+import host_twin
 import tracker_fixtures as tf
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 NQ, HIDDEN, CLASSES = 20, 32, 20
 
 
@@ -83,10 +80,7 @@ def blobs(det, seq_id, n_frames, scene_public, device="cpu"):
 
 
 def build_host(tmp, name):
-    so = str(tmp / f"lib{name}.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", f"{name}.cpp"), "-o", so])
-    return ctypes.CDLL(so)
+    return host_twin.build(name, tmp)
 
 
 def output_spans(a):

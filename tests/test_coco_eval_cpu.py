@@ -10,7 +10,6 @@ import ctypes
 import json
 import os
 import pickle
-import subprocess
 
 import numpy as np
 import pytest
@@ -18,17 +17,14 @@ import torch
 
 import coco_eval_fixtures as cf
 import coco_eval_reference as ref
+import host_twin
 from trackformer_b200 import coco_eval as ce
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope="module")
 def host_lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("coco_eval") / "libcoco_eval_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", "coco_eval_host.cpp"), "-o", so])
-    lib = ctypes.CDLL(so)
+    lib = host_twin.build("coco_eval_host", tmp_path_factory.mktemp("coco_eval"))
     vp, i32, i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
     lib.tfb200_coco_match_host.argtypes = ([vp, i32, i32, i32, vp, vp, vp, i64, vp, i32] + [vp] * 11
                                            + [i32, vp, i32, i32, i32, i64, i64, i64, i64, vp, vp, vp, vp, vp])

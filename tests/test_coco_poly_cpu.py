@@ -6,8 +6,6 @@ built here by g++ -ffp-contract=off with one "thread" (tests/host_build/coco_pol
 for run through the product's packing (`coco_masks.pack_polygons`) and error reporting (`coco_masks.check_sizes`).
 The CUDA build is compared in tests/test_coco_poly_gpu.py."""
 import ctypes
-import os
-import subprocess
 from fractions import Fraction
 
 import numpy as np
@@ -16,17 +14,14 @@ import pytest
 import coco_poly_fixtures as pf
 import coco_poly_reference as ref
 import eval_consistency_fixtures as ef
+import host_twin
 from trackformer_b200 import coco_eval, coco_masks, mots
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 @pytest.fixture(scope="module")
 def host_lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("coco_poly") / "libcoco_poly_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", "coco_poly_host.cpp"), "-o", so])
-    lib = ctypes.CDLL(so)
+    lib = host_twin.build("coco_poly_host", tmp_path_factory.mktemp("coco_poly"))
     vp, i32, i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64
     geo = [vp] * 5 + [i32, i32, i64]
     lib.tfb200_coco_poly_count_host.argtypes = geo + [vp, vp, vp]

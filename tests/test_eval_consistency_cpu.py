@@ -16,12 +16,12 @@ public CUDA entry points.  The checks are the `check_*` functions, written again
 import ctypes
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import eval_consistency_fixtures as ef
+import host_twin
 import mot_eval_fixtures as mf
 from test_coco_eval_cpu import host_eval
 from test_mot_eval_cpu import host_counters as mot_host_counters
@@ -29,17 +29,13 @@ from test_mots_eval_cpu import host_counters as mots_host_counters
 from trackformer_b200 import mot_eval, mots_eval
 from trackformer_b200 import panoptic_eval as pe
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 MOT_COUNTS = {"matches": mot_eval._MATCH, "switches": mot_eval._SWITCH, "misses": mot_eval._MISS,
               "fp": mot_eval._FP, "frag": mot_eval._FRAG, "mt": mot_eval._MT, "pt": mot_eval._PT,
               "ml": mot_eval._ML, "idtp": mot_eval._IDTP}
 
 
 def _compile(tmp_path_factory, name, argtypes):
-    so = str(tmp_path_factory.mktemp(name) / f"lib{name}_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", f"{name}_host.cpp"), "-o", so])
-    lib = ctypes.CDLL(so)
+    lib = host_twin.build(f"{name}_host", tmp_path_factory.mktemp(name))
     for fn, (args, res) in argtypes.items():
         getattr(lib, fn).argtypes, getattr(lib, fn).restype = args, res
     return lib
@@ -61,10 +57,8 @@ def host_lib(tmp_path_factory):
         "tfb200_mots_eval_host_workspace_bytes": ([i32, i32, i32, i64, i64, i64, i32, i32, i64, i64, i64], sz),
         "tfb200_mots_eval_host": ([vp] * 9 + [i32, i32, i32, i64, i64, i64, i32, i32, i64, i64, i64, vp, sz, vp],
                                   i32)})
-    so = str(tmp_path_factory.mktemp("panoptic") / "libpanoptic_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", "panoptic_host.cpp"), "-o", so])
-    return {"coco": coco, "mot": mot, "mots": mots, "pq": pe.bind(ctypes.CDLL(so))}
+    pq = pe.bind(host_twin.build("panoptic_host", tmp_path_factory.mktemp("panoptic")))
+    return {"coco": coco, "mot": mot, "mots": mots, "pq": pq}
 
 
 class HostBackend:

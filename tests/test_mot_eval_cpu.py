@@ -6,29 +6,24 @@ csrc/mot_eval.cu's kernels are compiled from, built here by g++ with one "thread
 summary (`summarize`).  Also: both GT box formats, the pickle round trip, the C entry's argument checks and the
 rendering of `str_summary`.  The CUDA build of the same source is compared in tests/test_mot_eval_gpu.py."""
 import ctypes
-import os
 import pickle
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import host_twin
 import mot_eval_fixtures as mf
 import mot_eval_reference as ref
 from trackformer_b200 import mot_eval
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 INTS = ("num_unique_objects", "mostly_tracked", "partially_tracked", "mostly_lost", "num_false_positives",
         "num_misses", "num_switches", "num_fragmentations")
 
 
 @pytest.fixture(scope="module")
 def host_lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("mot_eval") / "libmot_eval_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", "mot_eval_host.cpp"), "-o", so])
-    lib = ctypes.CDLL(so)
+    lib = host_twin.build("mot_eval_host", tmp_path_factory.mktemp("mot_eval"))
     i32, i64, vp = ctypes.c_int, ctypes.c_int64, ctypes.c_void_p
     lib.tfb200_mot_eval_host_workspace_bytes.argtypes = [i32, i32, i64, i64, i64, i32, i32, i64]
     lib.tfb200_mot_eval_host_workspace_bytes.restype = ctypes.c_size_t

@@ -6,29 +6,24 @@ with one "thread" (tests/host_build/mots_eval_host.cpp) -- is compared with the 
 (`get_mots_accum`) and summary (`summarize`).  Also: the string decoder against `mots.decode_counts`, the MOTS20 file
 round trip, the pickle round trip, and every error class.  The CUDA build is compared in tests/test_mots_eval_gpu.py."""
 import ctypes
-import os
 import pickle
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import host_twin
 import mots_eval_fixtures as msf
 import mots_eval_reference as ref
 from trackformer_b200 import mots, mots_eval
 
-HERE = os.path.dirname(os.path.abspath(__file__))
 INTS = ("num_unique_objects", "mostly_tracked", "partially_tracked", "mostly_lost", "num_detections",
         "num_false_positives", "num_misses", "num_switches", "num_fragmentations", "num_ignored")
 
 
 @pytest.fixture(scope="module")
 def host_lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("mots_eval") / "libmots_eval_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", "mots_eval_host.cpp"), "-o", so])
-    lib = ctypes.CDLL(so)
+    lib = host_twin.build("mots_eval_host", tmp_path_factory.mktemp("mots_eval"))
     i32, i64, vp = ctypes.c_int, ctypes.c_int64, ctypes.c_void_p
     lib.tfb200_mots_eval_host_workspace_bytes.argtypes = [i32, i32, i32, i64, i64, i64, i32, i32, i64, i64, i64]
     lib.tfb200_mots_eval_host_workspace_bytes.restype = ctypes.c_size_t

@@ -5,17 +5,16 @@ csrc/panoptic_core.h -- the routines csrc/panoptic.cu's kernels are compiled fro
 host code with CPU tensors: `PostProcessPanoptic.label_maps` against the reference's fixtures
 (tests/golden/panoptic_postprocess.npz), and `PQScorer` / `pq_compute` against the numpy oracle
 (tests/panoptic_eval_reference.py), which is first pinned on hand-worked scenes."""
-import ctypes
 import io
 import json
 import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 from PIL import Image
 
+import host_twin
 import panoptic_eval_reference as ref
 import panoptic_fixtures as pf
 from trackformer_b200 import panoptic_eval as pe
@@ -29,10 +28,7 @@ IS_THING = {i: i <= 90 for i in range(201)}
 
 @pytest.fixture(scope="module")
 def host_lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("panoptic") / "libpanoptic_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", "panoptic_host.cpp"), "-o", so])
-    return pe.bind(ctypes.CDLL(so))
+    return pe.bind(host_twin.build("panoptic_host", tmp_path_factory.mktemp("panoptic")))
 
 
 def golden_case(name):

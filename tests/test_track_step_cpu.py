@@ -14,8 +14,9 @@ import numpy as np
 import pytest
 import torch
 
-import tracker_fixtures as tf
+import host_twin
 from test_tracker_cpu import check_against_gold
+import tracker_fixtures as tf
 from trackformer_b200.deformable_detr import DeformablePostProcess
 from trackformer_b200.device_tracker import DeviceTracker, _ArgsC
 from trackformer_b200.tracker import Tracker
@@ -26,10 +27,7 @@ GOLD = os.path.join(HERE, "golden")
 
 @pytest.fixture(scope="module")
 def host_tracker(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("track_step") / "libtrack_step_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", "track_step_host.cpp"), "-o", so])
-    lib = ctypes.CDLL(so)
+    lib = host_twin.build("track_step_host", tmp_path_factory.mktemp("track_step"))
     lib.tfb200_track_step_host.argtypes = [ctypes.POINTER(_ArgsC)]
     lib.tfb200_track_step_host.restype = ctypes.c_int
 

@@ -7,14 +7,14 @@ branch runs its CPU route (the reference's torch ops).
 """
 import ctypes
 import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-import two_stage_fixtures as tf
 from conftest import load_golden
+import host_twin
+import two_stage_fixtures as tf
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
@@ -111,10 +111,7 @@ def test_train_step_refuses_two_stage_segmentation():
 # ---- host build of the kernels' routines --------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def host_lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("two_stage_host") / "two_stage_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-ffp-contract=off", "-fPIC", "-shared",
-                           os.path.join(HERE, "host_build", "two_stage_host.cpp"), "-o", so])
-    lib = ctypes.CDLL(so)
+    lib = host_twin.build("two_stage_host", tmp_path_factory.mktemp("two_stage_host"))
     lib.tfb200_two_stage_proposals_host.restype = ctypes.c_int
     lib.tfb200_two_stage_select_host.restype = ctypes.c_int
     return lib

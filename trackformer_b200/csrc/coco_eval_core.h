@@ -25,44 +25,7 @@
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
-
-#if defined(__CUDACC__)
-#define CE_FN __device__ inline
-#define CE_SYNC() __syncthreads()
-#define CE_TID (int(threadIdx.x))
-#define CE_NT (int(blockDim.x))
-#define ce_add(a, b) __dadd_rn((a), (b))
-#define ce_sub(a, b) __dsub_rn((a), (b))
-#define ce_mul(a, b) __dmul_rn((a), (b))
-#define ce_div(a, b) __ddiv_rn((a), (b))
-#define ce_popc(v) __popc(v)
-#define ce_ctz(v) (__ffs(int(v)) - 1)
-#define ce_clz(v) __clz(int(v))
-__device__ inline void ce_or(uint32_t* p, uint32_t v) { atomicOr(reinterpret_cast<unsigned*>(p), unsigned(v)); }
-__device__ inline void ce_min(int* p, int v) { atomicMin(p, v); }
-__device__ inline void ce_max(int* p, int v) { atomicMax(p, v); }
-__device__ inline void ce_addll(long long* p, long long v) {
-  atomicAdd(reinterpret_cast<unsigned long long*>(p), static_cast<unsigned long long>(v));
-}
-__device__ inline void ce_maxu64(unsigned long long* p, unsigned long long v) { atomicMax(p, v); }
-#else
-#define CE_FN static inline
-#define CE_SYNC() ((void)0)
-#define CE_TID 0
-#define CE_NT 1
-#define ce_add(a, b) ((a) + (b))
-#define ce_sub(a, b) ((a) - (b))
-#define ce_mul(a, b) ((a) * (b))
-#define ce_div(a, b) ((a) / (b))
-#define ce_popc(v) __builtin_popcount(v)
-#define ce_ctz(v) __builtin_ctz(v)
-#define ce_clz(v) __builtin_clz(v)
-static inline void ce_or(uint32_t* p, uint32_t v) { *p |= v; }
-static inline void ce_min(int* p, int v) { if (v < *p) *p = v; }
-static inline void ce_max(int* p, int v) { if (v > *p) *p = v; }
-static inline void ce_addll(long long* p, long long v) { *p += v; }
-static inline void ce_maxu64(unsigned long long* p, unsigned long long v) { if (v > *p) *p = v; }
-#endif
+#include "host_device.h"
 
 namespace tfb200_coco {
 
@@ -135,34 +98,20 @@ struct AccParams {
 };
 
 // ---- scores ----
-CE_FN uint32_t ce_fbits(float f) {
-#if defined(__CUDACC__)
-  return uint32_t(__float_as_uint(f));
-#else
-  union { float f; uint32_t u; } c; c.f = f; return c.u;
-#endif
-}
-CE_FN float ce_bitsf(uint32_t u) {
-#if defined(__CUDACC__)
-  return __uint_as_float(u);
-#else
-  union { float f; uint32_t u; } c; c.u = u; return c.f;
-#endif
-}
 // Ascending in the result = descending in the score; -0 and +0 tie.
-CE_FN uint32_t ce_desc_bits(float s) {
-  uint32_t u = ce_fbits(s + 0.0f);
+HD_FN uint32_t ce_desc_bits(float s) {
+  uint32_t u = hd_float_bits(s + 0.0f);
   u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
   return ~u;
 }
-CE_FN float ce_desc_score(uint32_t d) {
+HD_FN float ce_desc_score(uint32_t d) {
   uint32_t u = ~d;
   u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
-  return ce_bitsf(u);
+  return hd_bits_float(u);
 }
-CE_FN bool ce_finite(float s) { return (ce_fbits(s) & 0x7f800000u) != 0x7f800000u; }
+HD_FN bool ce_finite(float s) { return (hd_float_bits(s) & 0x7f800000u) != 0x7f800000u; }
 
-CE_FN int ce_cat_index(const int64_t* cat_ids, int K, int64_t cat) {
+HD_FN int ce_cat_index(const int64_t* cat_ids, int K, int64_t cat) {
   int lo = 0, hi = K;
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
@@ -172,7 +121,7 @@ CE_FN int ce_cat_index(const int64_t* cat_ids, int K, int64_t cat) {
 }
 
 // The image's ground-truth rows [b, e) of category k (rows are sorted by category index).
-CE_FN void ce_gt_range(const MatchParams& p, int64_t gi, int k, int64_t& b, int64_t& e) {
+HD_FN void ce_gt_range(const MatchParams& p, int64_t gi, int k, int64_t& b, int64_t& e) {
   int64_t lo = p.gt_off[gi], hi = p.gt_off[gi + 1];
   int64_t l = lo, h = hi;
   while (l < h) { const int64_t m = (l + h) >> 1; if (p.gt_k[m] < k) l = m + 1; else h = m; }
@@ -182,43 +131,43 @@ CE_FN void ce_gt_range(const MatchParams& p, int64_t gi, int k, int64_t& b, int6
 }
 
 // ---- pycocotools maskApi.c bbIou: [x, y, w, h] in fp64, separately rounded ----
-CE_FN double ce_bb_iou(const double* d, const double* g, bool crowd) {
-  const double da = ce_mul(d[2], d[3]), ga = ce_mul(g[2], g[3]);
-  const double dx1 = ce_add(d[2], d[0]), gx1 = ce_add(g[2], g[0]);
-  const double w = ce_sub(dx1 < gx1 ? dx1 : gx1, d[0] > g[0] ? d[0] : g[0]);
+HD_FN double ce_bb_iou(const double* d, const double* g, bool crowd) {
+  const double da = hd_dmul(d[2], d[3]), ga = hd_dmul(g[2], g[3]);
+  const double dx1 = hd_dadd(d[2], d[0]), gx1 = hd_dadd(g[2], g[0]);
+  const double w = hd_dsub(dx1 < gx1 ? dx1 : gx1, d[0] > g[0] ? d[0] : g[0]);
   if (!(w > 0.0)) return 0.0;
-  const double dy1 = ce_add(d[3], d[1]), gy1 = ce_add(g[3], g[1]);
-  const double h = ce_sub(dy1 < gy1 ? dy1 : gy1, d[1] > g[1] ? d[1] : g[1]);
+  const double dy1 = hd_dadd(d[3], d[1]), gy1 = hd_dadd(g[3], g[1]);
+  const double h = hd_dsub(dy1 < gy1 ? dy1 : gy1, d[1] > g[1] ? d[1] : g[1]);
   if (!(h > 0.0)) return 0.0;
-  const double i = ce_mul(w, h);
-  const double u = crowd ? da : ce_sub(ce_add(da, ga), i);
-  return ce_div(i, u);
+  const double i = hd_dmul(w, h);
+  const double u = crowd ? da : hd_dsub(hd_dadd(da, ga), i);
+  return hd_ddiv(i, u);
 }
 
 // The detection box as convert_to_xywh makes it: w = x1 - x0 in float32, then widened.
-CE_FN void ce_dt_xywh(const float* b, double* o) {
+HD_FN void ce_dt_xywh(const float* b, double* o) {
   o[0] = double(b[0]); o[1] = double(b[1]);
   o[2] = double(float(b[2] - b[0])); o[3] = double(float(b[3] - b[1]));
 }
 
 // ---- 1. category, rank, key, order (one CTA per image) ----
-CE_FN void ce_rank(const MatchParams& p, int b) {
+HD_FN void ce_rank(const MatchParams& p, int b) {
   const int64_t* im = p.img + int64_t(b) * kImgFields;
   const int64_t d0 = im[kDetBegin];
   const int n = int(im[kDetCount]);
-  for (int j = CE_TID; j < n; j += CE_NT) {
+  for (int j = HD_TID; j < n; j += HD_NT) {
     const float s = p.scores[d0 + j];
     int k = ce_cat_index(p.cat_ids, p.K, p.labels[d0 + j] + 1);
     if (!ce_finite(s)) {
       k = -1;
-      ce_or(reinterpret_cast<uint32_t*>(p.status), kErrScore);
+      hd_atomic_or(reinterpret_cast<uint32_t*>(p.status), kErrScore);
     }
     p.dk[d0 + j] = k;
     p.dord[d0 + j] = -1;
     for (int a = 0; a < p.A; ++a) p.state[(d0 + j) * p.A + a] = 0;
   }
-  CE_SYNC();
-  for (int j = CE_TID; j < n; j += CE_NT) {
+  HD_SYNC();
+  for (int j = HD_TID; j < n; j += HD_NT) {
     const int k = p.dk[d0 + j];
     int r = INT32_MAX;
     if (k >= 0) {
@@ -242,12 +191,12 @@ CE_FN void ce_rank(const MatchParams& p, int b) {
   }
 }
 
-CE_FN bool ce_evaluated(const MatchParams& p, int64_t row) { return (p.key[row] >> 32) < uint64_t(p.K); }
+HD_FN bool ce_evaluated(const MatchParams& p, int64_t row) { return (p.key[row] >> 32) < uint64_t(p.K); }
 
 // ---- 2. segm: pack one detection's mask (one CTA per image x detection) ----
 struct PackShared { long long px; int x0, y0, x1, y1; };
 
-CE_FN void ce_pack_dt(const MatchParams& p, int b, int j, PackShared& sh) {
+HD_FN void ce_pack_dt(const MatchParams& p, int b, int j, PackShared& sh) {
   const int64_t* im = p.img + int64_t(b) * kImgFields;
   if (j >= im[kDetCount]) return;
   const int64_t row = im[kDetBegin] + j;
@@ -256,27 +205,27 @@ CE_FN void ce_pack_dt(const MatchParams& p, int b, int j, PackShared& sh) {
   const int64_t plane = int64_t(Hw) * W;
   const uint8_t* m = reinterpret_cast<const uint8_t*>(im[kMaskPtr]) + int64_t(j) * H * W;
   uint32_t* bits = p.dbits + im[kDbitsOff] + int64_t(j) * plane;
-  if (CE_TID == 0) { sh.px = 0; sh.x0 = INT_MAX; sh.y0 = INT_MAX; sh.x1 = -1; sh.y1 = -1; }
-  CE_SYNC();
+  if (HD_TID == 0) { sh.px = 0; sh.x0 = INT_MAX; sh.y0 = INT_MAX; sh.x1 = -1; sh.y1 = -1; }
+  HD_SYNC();
   long long px = 0;
   int x0 = INT_MAX, y0 = INT_MAX, x1 = -1, y1 = -1;
-  for (int64_t w = CE_TID; w < plane; w += CE_NT) {
+  for (int64_t w = HD_TID; w < plane; w += HD_NT) {
     const int x = int(w % W), wy = int(w / W);
     const int rows = H - 32 * wy < 32 ? H - 32 * wy : 32;
     uint32_t v = 0;
     for (int i = 0; i < rows; ++i) v |= uint32_t(m[int64_t(32 * wy + i) * W + x] != 0) << i;
     bits[w] = v;
     if (v) {
-      px += ce_popc(v);
+      px += hd_popc(v);
       x0 = x < x0 ? x : x0; x1 = x > x1 ? x : x1;
-      const int ya = 32 * wy + ce_ctz(v), yb = 32 * wy + 31 - ce_clz(v);
+      const int ya = 32 * wy + hd_ctz(v), yb = 32 * wy + 31 - hd_clz(v);
       y0 = ya < y0 ? ya : y0; y1 = yb > y1 ? yb : y1;
     }
   }
-  ce_addll(&sh.px, px);
-  ce_min(&sh.x0, x0); ce_min(&sh.y0, y0); ce_max(&sh.x1, x1); ce_max(&sh.y1, y1);
-  CE_SYNC();
-  if (CE_TID == 0) {
+  hd_atomic_add(&sh.px, px);
+  hd_atomic_min(&sh.x0, x0); hd_atomic_min(&sh.y0, y0); hd_atomic_max(&sh.x1, x1); hd_atomic_max(&sh.y1, y1);
+  HD_SYNC();
+  if (HD_TID == 0) {
     p.dpx[row] = sh.px;
     int32_t* bx = p.dbox + row * 4;
     bx[0] = sh.x0; bx[1] = sh.y0; bx[2] = sh.x1; bx[3] = sh.y1;
@@ -284,14 +233,14 @@ CE_FN void ce_pack_dt(const MatchParams& p, int b, int j, PackShared& sh) {
 }
 
 // ---- 3. segm: one ground truth's runs into its bit plane (zeroed before; one CTA per image x GT) ----
-CE_FN void ce_decode_gt(const MatchParams& p, int b, int g) {
+HD_FN void ce_decode_gt(const MatchParams& p, int b, int g) {
   const int64_t* im = p.img + int64_t(b) * kImgFields;
   const int64_t gi = im[kGtImg], gb = p.gt_off[gi];
   if (g >= p.gt_off[gi + 1] - gb) return;
   const int64_t row = gb + g;
   const int H = int(im[kH]), W = int(im[kW]), Hw = (H + 31) >> 5;
   uint32_t* bits = p.gbits + im[kGbitsOff] + int64_t(g) * Hw * W;
-  for (int64_t r = p.gt_run_off[row] + CE_TID; r < p.gt_run_off[row + 1]; r += CE_NT) {
+  for (int64_t r = p.gt_run_off[row] + HD_TID; r < p.gt_run_off[row + 1]; r += HD_NT) {
     int64_t t = p.gt_runs[2 * r], len = p.gt_runs[2 * r + 1];
     while (len > 0) {
       const int x = int(t / H), y = int(t % H);
@@ -300,7 +249,7 @@ CE_FN void ce_decode_gt(const MatchParams& p, int b, int g) {
         const int lo = y > 32 * wy ? y - 32 * wy : 0;
         const int hi = y + cnt - 32 * wy < 32 ? y + cnt - 32 * wy : 32;       // exclusive
         const uint32_t mk = (hi == 32 ? 0xffffffffu : ((1u << hi) - 1u)) & ~((1u << lo) - 1u);
-        ce_or(bits + int64_t(wy) * W + x, mk);
+        hd_atomic_or(bits + int64_t(wy) * W + x, mk);
       }
       t += cnt; len -= cnt;
     }
@@ -310,7 +259,7 @@ CE_FN void ce_decode_gt(const MatchParams& p, int b, int g) {
 // ---- 4. IoU of one detection against the image's ground truths of its category ----
 struct IouShared { long long inter; };
 
-CE_FN void ce_iou(const MatchParams& p, int b, int j, IouShared& sh) {
+HD_FN void ce_iou(const MatchParams& p, int b, int j, IouShared& sh) {
   const int64_t* im = p.img + int64_t(b) * kImgFields;
   if (j >= im[kDetCount]) return;
   const int64_t row = im[kDetBegin] + j;
@@ -322,7 +271,7 @@ CE_FN void ce_iou(const MatchParams& p, int b, int j, IouShared& sh) {
   if (!p.segm) {
     double d[4];
     ce_dt_xywh(p.boxes + row * 4, d);
-    for (int64_t g = g0 + CE_TID; g < g1; g += CE_NT) out[g] = ce_bb_iou(d, p.gt_box + g * 4, p.gt_crowd[g] != 0);
+    for (int64_t g = g0 + HD_TID; g < g1; g += HD_NT) out[g] = ce_bb_iou(d, p.gt_box + g * 4, p.gt_crowd[g] != 0);
     return;
   }
   const int H = int(im[kH]), W = int(im[kW]), Hw = (H + 31) >> 5;
@@ -334,39 +283,39 @@ CE_FN void ce_iou(const MatchParams& p, int b, int j, IouShared& sh) {
     const int x0 = bx[0] > gx[0] ? bx[0] : gx[0], x1 = bx[2] < gx[2] ? bx[2] : gx[2];
     const int y0 = bx[1] > gx[1] ? bx[1] : gx[1], y1 = bx[3] < gx[3] ? bx[3] : gx[3];
     if (x0 > x1 || y0 > y1) {                       // disjoint boxes (or an empty mask): IoU 0
-      if (CE_TID == 0) out[g] = 0.0;
+      if (HD_TID == 0) out[g] = 0.0;
       continue;
     }
     const uint32_t* gbits = p.gbits + im[kGbitsOff] + (g - gbase) * plane;
     const int nx = x1 - x0 + 1, w0 = y0 >> 5, nw = (y1 >> 5) - w0 + 1;
-    if (CE_TID == 0) sh.inter = 0;
-    CE_SYNC();
+    if (HD_TID == 0) sh.inter = 0;
+    HD_SYNC();
     long long c = 0;
-    for (int q = CE_TID; q < nx * nw; q += CE_NT) {
+    for (int q = HD_TID; q < nx * nw; q += HD_NT) {
       const int64_t w = int64_t(w0 + q / nx) * W + x0 + q % nx;
-      c += ce_popc(db[w] & gbits[w]);
+      c += hd_popc(db[w] & gbits[w]);
     }
-    ce_addll(&sh.inter, c);
-    CE_SYNC();
-    if (CE_TID == 0) {
+    hd_atomic_add(&sh.inter, c);
+    HD_SYNC();
+    if (HD_TID == 0) {
       const long long i = sh.inter;
       const long long u = p.gt_crowd[g] ? p.dpx[row] : p.dpx[row] + p.gt_px[g] - i;
-      out[g] = i == 0 ? 0.0 : ce_div(double(i), double(u));
+      out[g] = i == 0 ? 0.0 : hd_ddiv(double(i), double(u));
     }
-    CE_SYNC();
+    HD_SYNC();
   }
 }
 
 // ---- 5. evaluateImg (one CTA per image; gtm zeroed before) ----
-CE_FN bool ce_outside(double v, const double* rng) { return v < rng[0] || v > rng[1]; }
+HD_FN bool ce_outside(double v, const double* rng) { return v < rng[0] || v > rng[1]; }
 
-CE_FN void ce_match(const MatchParams& p, int b) {
+HD_FN void ce_match(const MatchParams& p, int b) {
   const int64_t* im = p.img + int64_t(b) * kImgFields;
   const int64_t d0 = im[kDetBegin];
   const int n = int(im[kDetCount]);
   const int64_t gi = im[kGtImg], gbase = p.gt_off[gi], ng = p.gt_off[gi + 1] - gbase;
   const int AT = p.A * p.T;
-  for (int64_t task = CE_TID; task < int64_t(n) * AT; task += CE_NT) {
+  for (int64_t task = HD_TID; task < int64_t(n) * AT; task += HD_NT) {
     const int pos = int(task / AT), a = int(task % AT) / p.T, t = int(task % p.T);
     const int j0 = p.dord[d0 + pos];
     if (j0 < 0) continue;
@@ -403,7 +352,7 @@ CE_FN void ce_match(const MatchParams& p, int b) {
         area = double(p.dpx[row]);
       } else {
         const float* bx = p.boxes + row * 4;
-        area = ce_mul(double(float(bx[2] - bx[0])), double(float(bx[3] - bx[1])));
+        area = hd_dmul(double(float(bx[2] - bx[0])), double(float(bx[3] - bx[1])));
       }
       uint32_t st;
       if (m >= 0) {
@@ -413,22 +362,22 @@ CE_FN void ce_match(const MatchParams& p, int b) {
       } else {
         st = ce_outside(area, rng) ? kIgnored : kFp;
       }
-      ce_or(p.state + row * p.A + a, st << (2 * t));
+      hd_atomic_or(p.state + row * p.A + a, st << (2 * t));
     }
   }
 }
 
 // ---- 6. accumulate ----
 // kept images' keys, in image-id order, with their record index as the sort value (one CTA per kept image)
-CE_FN void ce_gather(const AccParams& p, int i) {
+HD_FN void ce_gather(const AccParams& p, int i) {
   const int64_t* kp = p.kept + int64_t(i) * 3;
-  for (int64_t q = CE_TID; q < kp[2]; q += CE_NT) {
+  for (int64_t q = HD_TID; q < kp[2]; q += HD_NT) {
     p.key_in[kp[1] + q] = p.key[kp[0] + q];
     p.val_in[kp[1] + q] = kp[0] + q;
   }
 }
 
-CE_FN int64_t ce_lower(const uint64_t* a, int64_t n, uint64_t v) {
+HD_FN int64_t ce_lower(const uint64_t* a, int64_t n, uint64_t v) {
   int64_t lo = 0, hi = n;
   while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (a[m] < v) lo = m + 1; else hi = m; }
   return lo;
@@ -445,29 +394,29 @@ struct AccShared {
 // sorted stably).  pr[i] is counted towards q[r] for every r whose recall threshold tp[i] reaches, so the envelope
 // max_{i' >= i_r} pr[i'] is a maximum over recall indices; scores[r] is the score at i_r, the detection that makes
 // tp reach tq[r] (the first detection when tq[r] = 0).
-CE_FN void ce_acc(const AccParams& p, int cta, AccShared& sh) {
+HD_FN void ce_acc(const AccParams& p, int cta, AccShared& sh) {
   const int t = cta % p.T, m = (cta / p.T) % p.M, a = (cta / (p.T * p.M)) % p.A, k = cta / (p.T * p.M * p.A);
   const int R = p.R, K = p.K, A = p.A, M = p.M;
   const int64_t npig = p.npig[k * A + a];
   auto at5 = [&](int r) { return ((((int64_t(t) * R + r) * K + k) * A + a) * M + m); };
   const int64_t at4 = ((int64_t(t) * K + k) * A + a) * M + m;
   if (npig == 0) {
-    for (int r = CE_TID; r < R; r += CE_NT) { p.precision[at5(r)] = -1.0; p.scores[at5(r)] = -1.0; }
-    if (CE_TID == 0) p.recall[at4] = -1.0;
+    for (int r = HD_TID; r < R; r += HD_NT) { p.precision[at5(r)] = -1.0; p.scores[at5(r)] = -1.0; }
+    if (HD_TID == 0) p.recall[at4] = -1.0;
     return;
   }
   const int64_t sb = ce_lower(p.key_out, p.n, uint64_t(k) << 32), se = ce_lower(p.key_out, p.n, uint64_t(k + 1) << 32);
   const int maxd = p.max_dets[m];
   const double dn = double(npig);
-  for (int r = CE_TID; r < R; r += CE_NT) {
+  for (int r = HD_TID; r < R; r += HD_NT) {
     long long lo = 0, hi = npig;                  // rc = x / npig is monotone in x and reaches 1 at npig
-    while (lo < hi) { const long long x = (lo + hi) >> 1; if (ce_div(double(x), dn) >= p.rec_thr[r]) hi = x; else lo = x + 1; }
+    while (lo < hi) { const long long x = (lo + hi) >> 1; if (hd_ddiv(double(x), dn) >= p.rec_thr[r]) hi = x; else lo = x + 1; }
     sh.tq[r] = lo;
     sh.best[r] = 0;
     sh.ss[r] = 0.0;
   }
-  const int64_t len = se - sb, per = (len + CE_NT - 1) / CE_NT;
-  const int64_t cb = sb + (per * CE_TID < len ? per * CE_TID : len), ce = sb + (per * (CE_TID + 1) < len ? per * (CE_TID + 1) : len);
+  const int64_t len = se - sb, per = (len + HD_NT - 1) / HD_NT;
+  const int64_t cb = sb + (per * HD_TID < len ? per * HD_TID : len), ce = sb + (per * (HD_TID + 1) < len ? per * (HD_TID + 1) : len);
   long long ltp = 0, lfp = 0, ln = 0;
   for (int64_t i = cb; i < ce; ++i) {
     const int64_t src = p.val_out[i];
@@ -476,11 +425,11 @@ CE_FN void ce_acc(const AccParams& p, int cta, AccShared& sh) {
     const uint32_t st = (p.state[src * A + a] >> (2 * t)) & 3u;
     ltp += st == kTp; lfp += st == kFp;
   }
-  sh.part_tp[CE_TID] = ltp; sh.part_fp[CE_TID] = lfp; sh.part_n[CE_TID] = ln;
-  CE_SYNC();
+  sh.part_tp[HD_TID] = ltp; sh.part_fp[HD_TID] = lfp; sh.part_n[HD_TID] = ln;
+  HD_SYNC();
   long long tp = 0, fp = 0, nb = 0, tp_all = 0, n_all = 0;
-  for (int q = 0; q < CE_NT; ++q) {
-    if (q < CE_TID) { tp += sh.part_tp[q]; fp += sh.part_fp[q]; nb += sh.part_n[q]; }
+  for (int q = 0; q < HD_NT; ++q) {
+    if (q < HD_TID) { tp += sh.part_tp[q]; fp += sh.part_fp[q]; nb += sh.part_n[q]; }
     tp_all += sh.part_tp[q]; n_all += sh.part_n[q];
   }
   const double eps = 2.220446049250313e-16;       // np.spacing(1)
@@ -491,12 +440,12 @@ CE_FN void ce_acc(const AccParams& p, int cta, AccShared& sh) {
     const bool first = nb == 0;
     tp += st == kTp; fp += st == kFp; ++nb;
     const double dtp = double(tp);
-    const double pr = ce_div(dtp, ce_add(ce_add(double(fp), dtp), eps));
+    const double pr = hd_ddiv(dtp, hd_dadd(hd_dadd(double(fp), dtp), eps));
     int lo = 0, hi = R;                           // recall indices reached: tq[r] <= tp, r < lo
     while (lo < hi) { const int mid = (lo + hi) >> 1; if (sh.tq[mid] <= tp) lo = mid + 1; else hi = mid; }
     if (lo > 0) {
       union { double d; unsigned long long u; } c; c.d = pr;
-      ce_maxu64(&sh.best[lo - 1], c.u);
+      hd_atomic_max(&sh.best[lo - 1], c.u);
     }
     if (st == kTp || first) {
       const double sc = double(ce_desc_score(uint32_t(p.key_out[i])));
@@ -506,8 +455,8 @@ CE_FN void ce_acc(const AccParams& p, int cta, AccShared& sh) {
         for (int r = 0; r < R && sh.tq[r] == 0; ++r) sh.ss[r] = sc;
     }
   }
-  CE_SYNC();
-  if (CE_TID == 0) {
+  HD_SYNC();
+  if (HD_TID == 0) {
     double run = 0.0;
     for (int r = R - 1; r >= 0; --r) {
       union { double d; unsigned long long u; } c; c.u = sh.best[r];
@@ -516,7 +465,7 @@ CE_FN void ce_acc(const AccParams& p, int cta, AccShared& sh) {
       p.precision[at5(r)] = reached ? run : 0.0;
       p.scores[at5(r)] = reached ? sh.ss[r] : 0.0;
     }
-    p.recall[at4] = n_all > 0 ? ce_div(double(tp_all), dn) : 0.0;
+    p.recall[at4] = n_all > 0 ? hd_ddiv(double(tp_all), dn) : 0.0;
   }
 }
 

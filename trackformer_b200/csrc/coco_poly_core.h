@@ -23,25 +23,12 @@
 #pragma once
 
 #include <limits.h>
+#include <math.h>
 #include <stddef.h>
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
-
-#if defined(__CUDACC__)
-#define CP_FN __device__ inline
-#define cp_add(a, b) __dadd_rn((a), (b))
-#define cp_sub(a, b) __dsub_rn((a), (b))
-#define cp_mul(a, b) __dmul_rn((a), (b))
-#define cp_div(a, b) __ddiv_rn((a), (b))
-#else
-#include <math.h>
-#define CP_FN static inline
-#define cp_add(a, b) ((a) + (b))
-#define cp_sub(a, b) ((a) - (b))
-#define cp_mul(a, b) ((a) * (b))
-#define cp_div(a, b) ((a) / (b))
-#endif
+#include "host_device.h"
 
 namespace tfb200_poly {
 
@@ -66,21 +53,21 @@ struct PolyParams {
 };
 
 // (int)(5 c + .5) with C's truncation toward zero; false when c is not finite or the value overflows an int
-CP_FN bool cp_grid(double c, int64_t* g) {
-  const double q = cp_add(cp_mul(kScale, c), 0.5);
+HD_FN bool cp_grid(double c, int64_t* g) {
+  const double q = hd_dadd(hd_dmul(kScale, c), 0.5);
   if (!(q > -kIntLimit && q < kIntLimit)) return false;
   *g = int64_t(q);
   return true;
 }
 
 // (int)q as x86-64's cvttsd2si computes it: NaN (the 0 / 0 slope of a zero-length edge) gives INT_MIN
-CP_FN int64_t cp_trunc(double q) {
+HD_FN int64_t cp_trunc(double q) {
   if (!(q > -kIntLimit - 1.0 && q < kIntLimit)) return INT_MIN;
   return int64_t(q);
 }
 
 // the part holding edge e: the last p with part_off[p] <= e
-CP_FN int cp_part_of(const PolyParams& P, int64_t e) {
+HD_FN int cp_part_of(const PolyParams& P, int64_t e) {
   int lo = 0, hi = P.n_parts;                        // part_off[lo] <= e < part_off[hi]
   while (hi - lo > 1) {
     const int mid = (lo + hi) >> 1;
@@ -96,7 +83,7 @@ struct Edge {
   bool flip, xmajor;
 };
 
-CP_FN Edge cp_edge(const PolyParams& P, int p, int64_t e) {
+HD_FN Edge cp_edge(const PolyParams& P, int p, int64_t e) {
   const int64_t b = e + 1 == P.part_off[p + 1] ? P.part_off[p] : e + 1;   // x[k] = x[0]
   int64_t xs = 0, ys = 0, xe = 0, ye = 0;
   cp_grid(P.xy[2 * e], &xs); cp_grid(P.xy[2 * e + 1], &ys);
@@ -111,29 +98,29 @@ CP_FN Edge cp_edge(const PolyParams& P, int p, int64_t e) {
     t = ys; ys = ye; ye = t;
   }
   E.xs = xs; E.ys = ys;
-  E.s = E.xmajor ? cp_div(double(ye - ys), double(E.dx)) : cp_div(double(xe - xs), double(E.dy));
+  E.s = E.xmajor ? hd_ddiv(double(ye - ys), double(E.dx)) : hd_ddiv(double(xe - xs), double(E.dy));
   E.n = (E.xmajor ? E.dx : E.dy) + 1;
   return E;
 }
 
-CP_FN void cp_point(const Edge& E, int64_t d, int64_t* u, int64_t* v) {
+HD_FN void cp_point(const Edge& E, int64_t d, int64_t* u, int64_t* v) {
   if (E.xmajor) {
     const int64_t t = E.flip ? E.dx - d : d;
     *u = t + E.xs;
-    *v = cp_trunc(cp_add(cp_add(double(E.ys), cp_mul(E.s, double(t))), 0.5));
+    *v = cp_trunc(hd_dadd(hd_dadd(double(E.ys), hd_dmul(E.s, double(t))), 0.5));
   } else {
     const int64_t t = E.flip ? E.dy - d : d;
     *v = t + E.ys;
-    *u = cp_trunc(cp_add(cp_add(double(E.xs), cp_mul(E.s, double(t))), 0.5));
+    *u = cp_trunc(hd_dadd(hd_dadd(double(E.xs), hd_dmul(E.s, double(t))), 0.5));
   }
 }
 
 // the toggle x * h + y of the pair (u0, v0) -> (u1, v1), or -1
-CP_FN int64_t cp_toggle(int64_t u0, int64_t v0, int64_t u1, int64_t v1, int64_t h, int64_t w) {
+HD_FN int64_t cp_toggle(int64_t u0, int64_t v0, int64_t u1, int64_t v1, int64_t h, int64_t w) {
   if (u1 == u0) return -1;
-  const double xd = cp_sub(cp_div(cp_add(double(u1 < u0 ? u1 : u1 - 1), 0.5), kScale), 0.5);
+  const double xd = hd_dsub(hd_ddiv(hd_dadd(double(u1 < u0 ? u1 : u1 - 1), 0.5), kScale), 0.5);
   if (floor(xd) != xd || xd < 0 || xd > double(w - 1)) return -1;
-  double yd = cp_sub(cp_div(cp_add(double(v1 < v0 ? v1 : v0), 0.5), kScale), 0.5);
+  double yd = hd_dsub(hd_ddiv(hd_dadd(double(v1 < v0 ? v1 : v0), 0.5), kScale), 0.5);
   if (yd < 0) yd = 0;
   else if (yd > double(h)) yd = double(h);
   return int64_t(xd) * h + int64_t(ceil(yd));
@@ -141,7 +128,7 @@ CP_FN int64_t cp_toggle(int64_t u0, int64_t v0, int64_t u1, int64_t v1, int64_t 
 
 // Edge e: validates its first vertex (status bit 1 not finite, 2 out of the int range; *ann = its annotation) and
 // returns its boundary-point count (0 when the edge cannot be walked).
-CP_FN int64_t cp_edge_points(const PolyParams& P, int64_t e, int* bad, int* ann) {
+HD_FN int64_t cp_edge_points(const PolyParams& P, int64_t e, int* bad, int* ann) {
   const int p = cp_part_of(P, e);
   *ann = P.part_ann[p];
   *bad = 0;
@@ -161,7 +148,7 @@ CP_FN int64_t cp_edge_points(const PolyParams& P, int64_t e, int* bad, int* ann)
 // Edge e's toggles: the pairs (previous point, point) for every point of the edge, the first point of the part
 // excepted.  Returns the count; kWrite stores them at key[at ..] with the part as value.
 template <bool kWrite>
-CP_FN int64_t cp_edge_toggles(const PolyParams& P, int64_t e, int64_t at, uint32_t* key, int32_t* val) {
+HD_FN int64_t cp_edge_toggles(const PolyParams& P, int64_t e, int64_t at, uint32_t* key, int32_t* val) {
   const int p = cp_part_of(P, e);
   const int a = P.part_ann[p];
   const int64_t h = P.ann_hw[2 * a], w = P.ann_hw[2 * a + 1];
@@ -191,7 +178,7 @@ CP_FN int64_t cp_edge_toggles(const PolyParams& P, int64_t e, int64_t at, uint32
 // Annotation a: its toggles key[seg[a] .. seg[a + 1]) sorted by position, val = their part; par [n_parts] zero on
 // entry for a's parts (left as the parts' final parities).  Counts the runs of the union, or writes them to run.
 template <bool kWrite>
-CP_FN int64_t cp_sweep(const PolyParams& P, int a, const int32_t* seg, const uint32_t* key, const int32_t* val,
+HD_FN int64_t cp_sweep(const PolyParams& P, int a, const int32_t* seg, const uint32_t* key, const int32_t* val,
                        uint8_t* par, uint32_t* run) {
   const int64_t hw = int64_t(P.ann_hw[2 * a]) * P.ann_hw[2 * a + 1];
   int64_t i = seg[a], n = 0, start = 0, cover = 0;
@@ -224,7 +211,7 @@ CP_FN int64_t cp_sweep(const PolyParams& P, int a, const int32_t* seg, const uin
 // malformed (a character outside '0' .. 'o', a value cut short or over 7 characters, a negative count, or counts that
 // do not sum to h * w).  kWrite stores the runs at run[0 ..].
 template <bool kWrite>
-CP_FN int64_t cp_rle_decode(const uint8_t* c, int64_t len, int64_t hw, uint32_t* run) {
+HD_FN int64_t cp_rle_decode(const uint8_t* c, int64_t len, int64_t hw, uint32_t* run) {
   int64_t pos = 0, c1 = 0, c2 = 0, n = 0;
   if (len == 0) return -1;
   for (int64_t j = 0, i = 0; j < len; ++i) {
@@ -250,7 +237,7 @@ CP_FN int64_t cp_rle_decode(const uint8_t* c, int64_t len, int64_t hw, uint32_t*
 }
 
 // Byte (y, x) of an H x W mask whose runs are run[b .. e)
-CP_FN uint8_t cp_mask_pixel(const uint32_t* run, int64_t b, int64_t e, int64_t H, int64_t y, int64_t x) {
+HD_FN uint8_t cp_mask_pixel(const uint32_t* run, int64_t b, int64_t e, int64_t H, int64_t y, int64_t x) {
   const int64_t i = x * H + y;
   int64_t lo = b, hi = e;                            // the first run starting after i
   while (lo < hi) {

@@ -4,8 +4,9 @@
 // scipy.optimize.linear_sum_assignment once per decoder layer (src/trackformer/models/matcher.py:104,127 -- six
 // device->host synchronisations per training step).  This kernel solves the same rectangular assignment problems
 // on the device: one CTA per (decoder layer, batch element) problem, queries x that element's ground-truth boxes,
-// by shortest augmenting paths with dual variables (the Jonker-Volgenant scheme scipy's solver is built on),
-// in double precision like scipy (which promotes the float32 cost matrix to float64).  The optimum of a cost matrix
+// by shortest augmenting paths with dual variables (the Jonker-Volgenant scheme scipy's solver is built on; lsa_core.h,
+// the solver the tracker and the MOT evaluators share), in double precision like scipy (which promotes the float32
+// cost matrix to float64).  The optimum of a cost matrix
 // without exact ties is unique, so the assignment equals scipy's; pairs are emitted sorted by query index, the order
 // linear_sum_assignment returns.  (With exact float ties the two solvers may pick different, equally optimal pairs.)
 //
@@ -18,130 +19,34 @@
 // tfb200_lsa_wide_f32 solves with the same routine over a global workspace: the cost block transposed to
 // [target][query], so that each row scan reads contiguous memory, and the column state (L2-resident at these sizes).
 #include <cuda_runtime.h>
-#include <float.h>
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
 #include "launch_counter.h"
+#include "lsa_core.h"
 
 namespace {
 
+namespace lsa = tfb200_lsa;
+
 constexpr int kLsaThreads = 256;
 
-struct MinKey {
-  double val;
-  int tie;    // 0: column unassigned (preferred on equal value), 1: assigned
-  int idx;
-};
-
-__device__ __forceinline__ bool better(const MinKey& a, const MinKey& b) {
-  if (a.val != b.val) return a.val < b.val;
-  if (a.tie != b.tie) return a.tie < b.tie;
-  return a.idx < b.idx;
-}
-
-__device__ __forceinline__ MinKey warp_min(MinKey k) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    MinKey other;
-    other.val = __shfl_xor_sync(0xffffffffu, k.val, o);
-    other.tie = __shfl_xor_sync(0xffffffffu, k.tie, o);
-    other.idx = __shfl_xor_sync(0xffffffffu, k.idx, o);
-    if (better(other, k)) k = other;
-  }
-  return k;
-}
-
-// The solver of one (layer, image) problem, shared by both kernels.  Column state (shortest, v, path, row4col, in_sc)
-// and row state (u, col4row, visited) live where the caller points them: shared memory in lsa_kernel, a global
-// workspace in lsa_wide_kernel.  Cost of (row i, column j) = C[j * cs + i * rs].  Every value is computed by the same
-// expression in both, and the minimum is taken under the total order of `better`, so both give the same pairs.
+// One (layer, image) problem, shared by both kernels: the solve, then the pairs sorted by query index (rank = number
+// of targets matched to a smaller query).  The solver state lives where the caller points it: shared memory in
+// lsa_kernel, a global workspace in lsa_wide_kernel.
 template <int NT>
-__device__ __forceinline__ void lsa_solve(const float* __restrict__ C, size_t cs, size_t rs, int nr, int nc,
-                                          double* shortest, double* v, double* u, int* path, int* row4col,
-                                          int* col4row, int* visited, unsigned char* in_sc, int64_t* __restrict__ src,
-                                          int64_t* __restrict__ tgt, size_t out0, int t0, int* __restrict__ status) {
-  __shared__ MinKey s_key[NT / 32];
-  __shared__ MinKey s_best;
-  __shared__ int s_i, s_sink, s_nvisited, s_fail;
-
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  for (int j = tid; j < nc; j += NT) { v[j] = 0.0; row4col[j] = -1; }
-  for (int i = tid; i < nr; i += NT) { u[i] = 0.0; col4row[i] = -1; }
-  if (tid == 0) s_fail = 0;
-  __syncthreads();
-
-  for (int cur = 0; cur < nr; ++cur) {
-    for (int j = tid; j < nc; j += NT) { shortest[j] = DBL_MAX; path[j] = -1; in_sc[j] = 0; }
-    if (tid == 0) { s_i = cur; s_sink = -1; s_nvisited = 0; }
-    __syncthreads();
-    double min_val = 0.0;
-    while (true) {
-      const int i = s_i;
-      if (tid == 0) visited[s_nvisited++] = i;
-      const double ui = u[i];
-      const float* Ci = C + size_t(i) * rs;
-      MinKey best{DBL_MAX, 1, INT32_MAX};
-      for (int j = tid; j < nc; j += NT) {
-        if (in_sc[j]) continue;
-        const double r = min_val + double(Ci[size_t(j) * cs]) - ui - v[j];
-        if (r < shortest[j]) { shortest[j] = r; path[j] = i; }
-        const MinKey cand{shortest[j], row4col[j] == -1 ? 0 : 1, j};
-        if (better(cand, best)) best = cand;
-      }
-      best = warp_min(best);
-      if (lane == 0) s_key[wid] = best;
-      __syncthreads();
-      if (wid == 0) {
-        MinKey kk = lane < NT / 32 ? s_key[lane] : MinKey{DBL_MAX, 1, INT32_MAX};
-        kk = warp_min(kk);
-        if (lane == 0) {
-          s_best = kk;
-          if (kk.val == DBL_MAX || kk.idx == INT32_MAX) { s_fail = 1; s_sink = 0; }   // infeasible (all +inf)
-          else {
-            in_sc[kk.idx] = 1;
-            if (row4col[kk.idx] == -1) s_sink = kk.idx; else s_i = row4col[kk.idx];
-          }
-        }
-      }
-      __syncthreads();
-      min_val = s_best.val;
-      if (s_sink != -1) break;
-    }
-    if (s_fail) break;
-    // ---- dual update
-    const int nvis = s_nvisited, sink = s_sink;
-    for (int t = tid; t < nvis; t += NT) {
-      const int i = visited[t];
-      if (i == cur) u[i] += min_val;
-      else u[i] += min_val - shortest[col4row[i]];
-    }
-    for (int j = tid; j < nc; j += NT)
-      if (in_sc[j]) v[j] -= min_val - shortest[j];
-    __syncthreads();
-    // ---- augment along the path (short: at most nvis hops)
-    if (tid == 0) {
-      int j = sink;
-      while (true) {
-        const int i = path[j];
-        row4col[j] = i;
-        const int prev = col4row[i];
-        col4row[i] = j;
-        j = prev;
-        if (i == cur) break;
-      }
-    }
-    __syncthreads();
-  }
-  if (s_fail) {
-    if (tid == 0) atomicExch(status, 2);
+__device__ __forceinline__ void lsa_problem(const lsa::Strided& cost, int nr, int nc, const lsa::Rows& R,
+                                            const lsa::Cols& C, int64_t* __restrict__ src, int64_t* __restrict__ tgt,
+                                            size_t out0, int t0, int* __restrict__ status) {
+  __shared__ typename lsa::Cta<NT>::Scratch scratch;
+  if (!lsa::solve<lsa::Cta<NT>>(nr, nc, cost, R, C, scratch)) {
+    if (threadIdx.x == 0) atomicExch(status, 2);   // infeasible (all +inf)
     return;
   }
-  // ---- emit pairs sorted by query index (rank = number of targets matched to a smaller query)
-  for (int i = tid; i < nr; i += NT) {
-    const int q = col4row[i];
+  for (int i = threadIdx.x; i < nr; i += NT) {
+    const int q = R.col4row[i];
     int rank = 0;
-    for (int o = 0; o < nr; ++o) rank += col4row[o] < q;
+    for (int o = 0; o < nr; ++o) rank += R.col4row[o] < q;
     src[out0 + rank] = q;
     tgt[out0 + rank] = t0 + i;
   }
@@ -165,10 +70,10 @@ lsa_kernel(const float* __restrict__ cost, const int* __restrict__ off, int64_t*
   int* path = reinterpret_cast<int*>(u + nr);                  // [nc]
   int* row4col = path + nc;                                    // [nc]
   int* col4row = row4col + nc;                                 // [nr]
-  int* visited = col4row + nr;                                 // [nr] rows in SR, in visiting order
-  unsigned char* in_sc = reinterpret_cast<unsigned char*>(visited + nr);   // [nc]
-  lsa_solve<kLsaThreads>(C, size_t(T), 1, nr, nc, shortest, v, u, path, row4col, col4row, visited, in_sc, src, tgt,
-                         size_t(k) * T + t0, t0, status);
+  int* visited = col4row + nr;                                 // [nr]
+  uint8_t* in_sc = reinterpret_cast<uint8_t*>(visited + nr);   // [nc]
+  lsa_problem<kLsaThreads>(lsa::Strided{C, 1, size_t(T)}, nr, nc, lsa::Rows{u, col4row, visited},
+                           lsa::Cols{shortest, v, path, row4col, in_sc}, src, tgt, size_t(k) * T + t0, t0, status);
 }
 
 // ---- wide problems: column state in a global workspace, cost transposed to [target][query] -----------------------
@@ -233,12 +138,12 @@ lsa_wide_kernel(const int* __restrict__ off, unsigned char* __restrict__ ws, int
   }
   const WideLayout l = wide_layout(Q, R);
   unsigned char* w = ws + size_t(p) * l.total;
-  lsa_solve<kWideThreads>(reinterpret_cast<const float*>(w + l.cost), 1, size_t(Q), nr, nc,
-                          reinterpret_cast<double*>(w + l.shortest), reinterpret_cast<double*>(w + l.v),
-                          reinterpret_cast<double*>(w + l.u), reinterpret_cast<int*>(w + l.path),
-                          reinterpret_cast<int*>(w + l.row4col), reinterpret_cast<int*>(w + l.col4row),
-                          reinterpret_cast<int*>(w + l.visited), w + l.in_sc, src, tgt, size_t(k) * T + t0, t0,
-                          status);
+  const lsa::Rows rows{reinterpret_cast<double*>(w + l.u), reinterpret_cast<int*>(w + l.col4row),
+                       reinterpret_cast<int*>(w + l.visited)};
+  const lsa::Cols cols{reinterpret_cast<double*>(w + l.shortest), reinterpret_cast<double*>(w + l.v),
+                       reinterpret_cast<int*>(w + l.path), reinterpret_cast<int*>(w + l.row4col), w + l.in_sc};
+  lsa_problem<kWideThreads>(lsa::Strided{reinterpret_cast<const float*>(w + l.cost), size_t(Q), 1}, nr, nc, rows,
+                            cols, src, tgt, size_t(k) * T + t0, t0, status);
 }
 
 }  // namespace

@@ -100,39 +100,31 @@ static inline size_t ms_carve(MsParams& p, char* ws, int S, int F, int n_masks, 
   return o + ((sort_bytes + 255) & ~size_t(255));
 }
 
-ME_FN void ms_min64(int64_t* p, int64_t v) {
-#if defined(__CUDACC__)
-  atomicMin(reinterpret_cast<long long*>(p), (long long)v);
-#else
-  if (v < *p) *p = v;
-#endif
-}
-
 // error `bit` in frame f (global): the status bit and the first such frame of f's sequence
-ME_FN void ms_flag(const MsParams& P, int64_t f, int bit) {
+HD_FN void ms_flag(const MsParams& P, int64_t f, int bit) {
   const int s = me_seq_of(P.core, kFrameBegin, f);
   int64_t* x = P.xout + int64_t(s) * kMsSlots;
-  me_or64(x + kMsStatus, bit);
+  hd_atomic_or(x + kMsStatus, bit);
   int b = 0;
   while ((1 << b) != bit) ++b;
-  ms_min64(x + kMsFirstFrame + b, f - P.core.seq[int64_t(s) * kSeqFields + kFrameBegin]);
+  hd_atomic_min(x + kMsFirstFrame + b, f - P.core.seq[int64_t(s) * kSeqFields + kFrameBegin]);
 }
 
-ME_FN int ms_side(const MsParams& P, int f, int m) {
+HD_FN int ms_side(const MsParams& P, int f, int m) {
   return m >= P.fm[3 * f + 2] ? kSideHyp : m >= P.fm[3 * f + 1] ? kSideIgnore : kSideGt;
 }
 
 // ---- per sequence ----
-ME_FN void ms_init_seq(const MsParams& P, int s) {
+HD_FN void ms_init_seq(const MsParams& P, int s) {
   me_init_seq(P.core, s);
   int64_t* x = P.xout + int64_t(s) * kMsSlots;
-  for (int k = ME_TID; k < kMsSlots; k += ME_NT) x[k] = k >= kMsFirstFrame ? INT64_MAX : 0;
+  for (int k = HD_TID; k < kMsSlots; k += HD_NT) x[k] = k >= kMsFirstFrame ? INT64_MAX : 0;
 }
 
 // ---- per mask m: decode its counts string.  Count pass: icount / area (0 for a bad mask, with the error flagged);
 // write pass: the intervals at ioff[m] .. ioff[m + 1] ----
 template <bool kWrite>
-ME_FN void ms_decode(const MsParams& P, int m) {
+HD_FN void ms_decode(const MsParams& P, int m) {
   const int32_t* mi = P.mask + int64_t(m) * kMaskFields;
   const int f = mi[kMaskFrame];
   int64_t at = 0, lim = 0;
@@ -188,7 +180,7 @@ ME_FN void ms_decode(const MsParams& P, int m) {
 }
 
 // ---- one CTA: interval offsets (all zero, capacity flagged everywhere, when they pass icap) and frame segments ----
-ME_FN void ms_scan_masks(const MsParams& P, Shared& sh) {
+HD_FN void ms_scan_masks(const MsParams& P, Shared& sh) {
   int64_t b, e;
   me_chunk(P.n_masks, b, e);
   int64_t v = 0;
@@ -196,15 +188,15 @@ ME_FN void ms_scan_masks(const MsParams& P, Shared& sh) {
   int64_t at = me_scan_parts(sh, v);
   const bool over = sh.base > P.icap;
   for (int64_t m = b; m < e; ++m) { P.ioff[m] = over ? 0 : int32_t(at); at += P.icount[m]; }
-  if (ME_TID == 0) P.ioff[P.n_masks] = over ? 0 : int32_t(sh.base);
-  ME_SYNC();
+  if (HD_TID == 0) P.ioff[P.n_masks] = over ? 0 : int32_t(sh.base);
+  HD_SYNC();
   const int F = P.core.F;
-  for (int f = ME_TID; f < F; f += ME_NT) {
+  for (int f = HD_TID; f < F; f += HD_NT) {
     P.segoff[2 * f] = P.ioff[P.fm[3 * f]];
     P.segoff[2 * f + 1] = P.ioff[P.fm[3 * f + 2]];
   }
-  if (ME_TID == 0) P.segoff[2 * F] = P.ioff[P.fm[3 * F]];
-  for (int s = ME_TID; s < P.core.S; s += ME_NT) {
+  if (HD_TID == 0) P.segoff[2 * F] = P.ioff[P.fm[3 * F]];
+  for (int s = HD_TID; s < P.core.S; s += HD_NT) {
     const int64_t* q = P.core.seq + int64_t(s) * kSeqFields;
     int64_t* x = P.xout + int64_t(s) * kMsSlots;
     x[kMsIntervals] = P.ioff[P.fm[3 * q[kFrameEnd]]] - P.ioff[P.fm[3 * q[kFrameBegin]]];
@@ -213,7 +205,7 @@ ME_FN void ms_scan_masks(const MsParams& P, Shared& sh) {
 }
 
 // the mask holding interval k < ioff[n_masks]: the last m with ioff[m] <= k (empty masks share the next offset)
-ME_FN int ms_mask_of(const MsParams& P, int64_t k) {
+HD_FN int ms_mask_of(const MsParams& P, int64_t k) {
   int lo = 0, hi = P.n_masks - 1;
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
@@ -224,7 +216,7 @@ ME_FN int ms_mask_of(const MsParams& P, int64_t k) {
 
 // ---- per sorted interval k: its end and GT row (the frame's GT count for an ignore mask); overlap with the previous
 // interval of its segment ----
-ME_FN void ms_gather(const MsParams& P, int64_t k) {
+HD_FN void ms_gather(const MsParams& P, int64_t k) {
   if (k >= P.ioff[P.n_masks]) return;
   const int src = P.sidx[k], m = ms_mask_of(P, src), f = P.mask[int64_t(m) * kMaskFields + kMaskFrame];
   const int side = ms_side(P, f, m);
@@ -236,7 +228,7 @@ ME_FN void ms_gather(const MsParams& P, int64_t k) {
 }
 
 // ---- per interval k (mask order): a hypothesis interval's overlaps with the frame's GT-side intervals ----
-ME_FN void ms_intersect(const MsParams& P, int64_t k) {
+HD_FN void ms_intersect(const MsParams& P, int64_t k) {
   if (k >= P.ioff[P.n_masks]) return;
   const int m = ms_mask_of(P, k), f = P.mask[int64_t(m) * kMaskFields + kMaskFrame];
   if (ms_side(P, f, m) != kSideHyp) return;
@@ -251,18 +243,18 @@ ME_FN void ms_intersect(const MsParams& P, int64_t k) {
   int32_t* cell = P.cell + P.fcell[f];
   for (int64_t j = lo; j < end && P.sstart[j] < e0; ++j) {
     const int32_t a = P.sstart[j] > s0 ? P.sstart[j] : s0, b = P.gs_end[j] < e0 ? P.gs_end[j] : e0;
-    if (b > a) me_atomic_add(cell + int64_t(P.gs_row[j]) * nh + h, b - a);
+    if (b > a) hd_atomic_add(cell + int64_t(P.gs_row[j]) * nh + h, b - a);
   }
 }
 
 // candidate pair: exact IoU >= 0.5 with a non-empty intersection
-ME_FN bool ms_cand(int64_t inter, int64_t uni) { return inter > 0 && 2 * inter >= uni; }
+HD_FN bool ms_cand(int64_t inter, int64_t uni) { return inter > 0 && 2 * inter >= uni; }
 
 // ---- per frame: candidates and the ignore rule.  Count pass: keep flags, fcount (valid pairs), kept hypotheses and
 // the sequence's counters; write pass: kept hypotheses' track ids at their compacted rows, the valid pairs (object,
 // then kept hypothesis) with d, and tp ----
 template <bool kWrite>
-ME_FN void ms_frame(const MsParams& P, int f, Shared& sh) {
+HD_FN void ms_frame(const MsParams& P, int f, Shared& sh) {
   const Params& C = P.core;
   if (kWrite && C.foff[C.F] > C.pair_cap) return;
   const int gb = P.fm[3 * f], no = P.fm[3 * f + 1] - gb, hb = P.fm[3 * f + 2], nh = P.fm[3 * f + 3] - hb;
@@ -270,7 +262,7 @@ ME_FN void ms_frame(const MsParams& P, int f, Shared& sh) {
   const int32_t *ga = P.area + gb, *ha = P.area + hb;
   if (!kWrite) {
     int64_t kept = 0, inters = 0;
-    for (int h = ME_TID; h < nh; h += ME_NT) {
+    for (int h = HD_TID; h < nh; h += HD_NT) {
       bool cand = false;
       for (int o = 0; o < no; ++o) {
         const int64_t in = cell[int64_t(o) * nh + h];
@@ -294,14 +286,14 @@ ME_FN void ms_frame(const MsParams& P, int f, Shared& sh) {
     me_scan_parts(sh, kept);
     const int64_t nk = sh.base;
     me_scan_parts(sh, inters);
-    if (ME_TID == 0) {
+    if (HD_TID == 0) {
       C.fcount[f] = int32_t(pairs);
       P.fcount_kept[f] = int32_t(nk);
       int64_t* x = P.xout + int64_t(me_seq_of(C, kFrameBegin, f)) * kMsSlots;
-      me_add64(x + kMsGtDets, no);
-      me_add64(x + kMsKept, nk);
-      me_add64(x + kMsRemoved, nh - nk);
-      me_add64(x + kMsIntersecting, sh.base);
+      hd_atomic_add(x + kMsGtDets, no);
+      hd_atomic_add(x + kMsKept, nk);
+      hd_atomic_add(x + kMsRemoved, nh - nk);
+      hd_atomic_add(x + kMsIntersecting, sh.base);
     }
     return;
   }
@@ -317,7 +309,7 @@ ME_FN void ms_frame(const MsParams& P, int f, Shared& sh) {
     P.hyp_id[P.fhyp[f] + r] = P.mask[int64_t(hb + h) * kMaskFields + kMaskId];
     ++r;
   }
-  ME_SYNC();
+  HD_SYNC();
   me_chunk(int64_t(no) * nh, b, e);
   int64_t cnt = 0;
   for (int64_t k = b; k < e; ++k) {
@@ -334,14 +326,14 @@ ME_FN void ms_frame(const MsParams& P, int f, Shared& sh) {
     if (!ms_cand(in, uni)) continue;
     const int row = P.fhyp[f] + P.keep[hb + h] - 1;
     C.pair_o[at] = C.fobj[f] + o; C.pair_h[at] = row;
-    C.pair_d[at] = me_sub(1.0, me_div(double(in), double(uni)));
+    C.pair_d[at] = hd_dsub(1.0, hd_ddiv(double(in), double(uni)));
     ++at;
-    me_atomic_add(tp + int64_t(C.obj_id[C.fobj[f] + o]) * H + P.hyp_id[row], 1);
+    hd_atomic_add(tp + int64_t(C.obj_id[C.fobj[f] + o]) * H + P.hyp_id[row], 1);
   }
 }
 
 // ---- one CTA: the pairs' frame offsets (me_scan) and the kept hypotheses' ----
-ME_FN void ms_scan(const MsParams& P, Shared& sh) {
+HD_FN void ms_scan(const MsParams& P, Shared& sh) {
   me_scan(P.core, sh);
   int64_t b, e;
   me_chunk(P.core.F, b, e);
@@ -349,8 +341,8 @@ ME_FN void ms_scan(const MsParams& P, Shared& sh) {
   for (int64_t f = b; f < e; ++f) v += P.fcount_kept[f];
   int64_t at = me_scan_parts(sh, v);
   for (int64_t f = b; f < e; ++f) { P.fhyp[f] = int32_t(at); at += P.fcount_kept[f]; }
-  if (ME_TID == 0) P.fhyp[P.core.F] = int32_t(sh.base);
-  ME_SYNC();
+  if (HD_TID == 0) P.fhyp[P.core.F] = int32_t(sh.base);
+  HD_SYNC();
 }
 
 }  // namespace tfb200_mots

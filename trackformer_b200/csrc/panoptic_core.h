@@ -26,37 +26,8 @@
 #include <stdint.h>
 
 #include "../../include/tfb200_fused.h"
+#include "host_device.h"
 #include "interp_index.h"
-
-#if defined(__CUDACC__)
-#define PN_FN __device__ inline
-#define PN_SYNC() __syncthreads()
-#define PN_TID (int(threadIdx.x))
-#define PN_NT (int(blockDim.x))
-#define pn_div(a, b) __fdiv_rn((a), (b))
-#define pn_add(a, b) __fadd_rn((a), (b))
-#define pn_sub(a, b) __fsub_rn((a), (b))
-#define pn_dadd(a, b) __dadd_rn((a), (b))
-#define pn_dsub(a, b) __dsub_rn((a), (b))
-#define pn_ddiv(a, b) __ddiv_rn((a), (b))
-__device__ inline void pn_add64(unsigned long long* p, unsigned long long v) { atomicAdd(p, v); }
-__device__ inline void pn_add32(int* p, int v) { atomicAdd(p, v); }
-__device__ inline void pn_min64(long long* p, long long v) { atomicMin(p, v); }
-#else
-#define PN_FN static inline
-#define PN_SYNC() ((void)0)
-#define PN_TID 0
-#define PN_NT 1
-#define pn_div(a, b) ((a) / (b))
-#define pn_add(a, b) ((a) + (b))
-#define pn_sub(a, b) ((a) - (b))
-#define pn_dadd(a, b) ((a) + (b))
-#define pn_dsub(a, b) ((a) - (b))
-#define pn_ddiv(a, b) ((a) / (b))
-static inline void pn_add64(unsigned long long* p, unsigned long long v) { *p += v; }
-static inline void pn_add32(int* p, int v) { *p += v; }
-static inline void pn_min64(long long* p, long long v) { if (v < *p) *p = v; }
-#endif
 
 namespace tfb200_panoptic {
 
@@ -104,17 +75,17 @@ struct PpParams {
   int32_t* out;                      // target-size maps (survivor position)
 };
 
-PN_FN void pp_classes(const PpParams& p, int64_t row) {
+HD_FN void pp_classes(const PpParams& p, int64_t row) {
   if (row >= int64_t(p.B) * p.Q) return;
   const float* x = p.logits + row * p.C;
   float m = x[0];
   for (int c = 1; c < p.C; ++c) m = x[c] > m ? x[c] : m;
   float s = 0.f;
-  for (int c = 0; c < p.C; ++c) s = pn_add(s, expf(pn_sub(x[c], m)));
+  for (int c = 0; c < p.C; ++c) s = hd_fadd(s, expf(hd_fsub(x[c], m)));
   float best = -1.f;
   int arg = 0;
   for (int c = 0; c < p.C; ++c) {
-    const float v = pn_div(expf(pn_sub(x[c], m)), s);
+    const float v = hd_fdiv(expf(hd_fsub(x[c], m)), s);
     if (v > best) { best = v; arg = c; }
   }
   p.cls[row] = arg;
@@ -123,7 +94,7 @@ PN_FN void pp_classes(const PpParams& p, int64_t row) {
 }
 
 // one CTA: pixels blk * kBlockPixels .. of image b; hist has kMaxKept entries (shared memory on the device)
-PN_FN void pp_label(const PpParams& p, int b, int blk, unsigned long long* hist) {
+HD_FN void pp_label(const PpParams& p, int b, int blk, unsigned long long* hist) {
   const int64_t* g = p.img + int64_t(b) * kPpFields;
   const int H = int(g[kPpH]), W = int(g[kPpW]), K = int(g[kPpK]);
   const int64_t npix = int64_t(H) * W, first = int64_t(blk) * kBlockPixels;
@@ -138,10 +109,10 @@ PN_FN void pp_label(const PpParams& p, int b, int blk, unsigned long long* hist)
   const bool dedup = g[kPpDedup] != 0;
   const int64_t plane = int64_t(p.h) * p.w;
   const float* mb = p.masks + int64_t(b) * p.Q * plane;
-  for (int k = PN_TID; k < K; k += PN_NT) hist[k] = 0ull;
-  PN_SYNC();
+  for (int k = HD_TID; k < K; k += HD_NT) hist[k] = 0ull;
+  HD_SYNC();
   const int64_t last = first + kBlockPixels < npix ? first + kBlockPixels : npix;
-  for (int64_t i = first + PN_TID; i < last; i += PN_NT) {
+  for (int64_t i = first + HD_TID; i < last; i += HD_NT) {
     const int y = int(i / W), x = int(i - int64_t(y) * W);
     const Lin ly = linear_src(y, p.h, H), lx = linear_src(x, p.w, W);
     // max and its first position, then the sum of expf(x - max), then the ties of the rounded probabilities
@@ -157,27 +128,27 @@ PN_FN void pp_label(const PpParams& p, int b, int blk, unsigned long long* hist)
     int cand = arg;
     for (int k = 0; k < K; ++k) {
       if (!alive[k]) continue;
-      const float e = expf(pn_sub(bilinear_at(mb + q[k] * plane, p.w, ly, lx), m));
-      s = pn_add(s, e);
+      const float e = expf(hd_fsub(bilinear_at(mb + q[k] * plane, p.w, ly, lx), m));
+      s = hd_fadd(s, e);
       if (k < cand && e > 0.99999f) cand = k;           // p_k can round equal to 1 / s only if e_k > 1 - 2^-20
     }
-    const float top = pn_div(1.f, s);
+    const float top = hd_fdiv(1.f, s);
     for (int k = cand; k < arg; ++k) {
       if (!alive[k]) continue;
-      const float e = expf(pn_sub(bilinear_at(mb + q[k] * plane, p.w, ly, lx), m));
-      if (pn_div(e, s) == top) { arg = k; break; }
+      const float e = expf(hd_fsub(bilinear_at(mb + q[k] * plane, p.w, ly, lx), m));
+      if (hd_fdiv(e, s) == top) { arg = k; break; }
     }
     const int lab = dedup ? rep[arg] : arg;
     map[i] = lab;
     const unsigned long long wgt = (unsigned long long)rcnt[y] * (unsigned long long)ccnt[x];
-    if (wgt) pn_add64(hist + lab, wgt);
+    if (wgt) hd_atomic_add(hist + lab, wgt);
   }
-  PN_SYNC();
-  for (int k = PN_TID; k < K; k += PN_NT)
-    if (hist[k]) pn_add64(p.area + ko + k, hist[k]);
+  HD_SYNC();
+  for (int k = HD_TID; k < K; k += HD_NT)
+    if (hist[k]) hd_atomic_add(p.area + ko + k, hist[k]);
 }
 
-PN_FN void pp_final(const PpParams& p, int b, int blk) {
+HD_FN void pp_final(const PpParams& p, int b, int blk) {
   const int64_t* g = p.img + int64_t(b) * kPpFields;
   const int W = int(g[kPpW]), Ht = int(g[kPpHt]), Wt = int(g[kPpWt]), K = int(g[kPpK]);
   const int64_t npix = int64_t(Ht) * Wt, first = int64_t(blk) * kBlockPixels;
@@ -190,7 +161,7 @@ PN_FN void pp_final(const PpParams& p, int b, int blk) {
   const int32_t* map = p.map + g[kPpMapOff];
   int32_t* out = p.out + g[kPpOutOff];
   const int64_t last = first + kBlockPixels < npix ? first + kBlockPixels : npix;
-  for (int64_t i = first + PN_TID; i < last; i += PN_NT) {
+  for (int64_t i = first + HD_TID; i < last; i += HD_NT) {
     const int y = int(i / Wt), x = int(i - int64_t(y) * Wt);
     out[i] = any ? p.kept_pos[ko + map[int64_t(rows[y]) * W + cols[x]]] : 0;
   }
@@ -230,7 +201,7 @@ struct PqParams {
   long long* err;                    // [rows][kErrFields] out
 };
 
-PN_FN int pq_find(const int32_t* ids, int n, int32_t v) {
+HD_FN int pq_find(const int32_t* ids, int n, int32_t v) {
   int lo = 0, hi = n;
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
@@ -240,7 +211,7 @@ PN_FN int pq_find(const int32_t* ids, int n, int32_t v) {
 }
 
 // one CTA: pixels blk * kBlockPixels .. of image b; sh has kSharedCells entries (shared memory on the device)
-PN_FN void pq_count(const PqParams& p, int b, int blk, int* sh) {
+HD_FN void pq_count(const PqParams& p, int b, int blk, int* sh) {
   const int64_t* g = p.img + int64_t(b) * kPqFields;
   const int64_t npix = g[kPqPix], first = int64_t(blk) * kBlockPixels;
   if (first >= npix) return;
@@ -255,25 +226,25 @@ PN_FN void pq_count(const PqParams& p, int b, int blk, int* sh) {
   const int32_t* pm = p.maps + g[kPqPredMap];
   long long* err = p.err + g[kPqStatRow] * kErrFields;
   if (in_sh) {
-    for (int c = PN_TID; c < ncell; c += PN_NT) sh[c] = 0;
-    PN_SYNC();
+    for (int c = HD_TID; c < ncell; c += HD_NT) sh[c] = 0;
+    HD_SYNC();
   }
   const int64_t last = first + kBlockPixels < npix ? first + kBlockPixels : npix;
-  for (int64_t i = first + PN_TID; i < last; i += PN_NT) {
+  for (int64_t i = first + HD_TID; i < last; i += HD_NT) {
     const int32_t gv = gm[i], pv = pm[i];
     int gr = pq_find(gid, G, gv);
     if (gr < 0) gr = gv == 0 ? void_row : G + 1;        // VOID, or an id the JSON does not list
     int pc = pq_find(pid, P, pv);
     if (pc < 0) {
-      if (pv != 0) { pn_min64(err + kErrUnlisted, (long long)pv); continue; }
+      if (pv != 0) { hd_atomic_min(err + kErrUnlisted, (long long)pv); continue; }
       pc = P;                                            // VOID
     }
-    pn_add32(acc + gr * (P + 1) + pc, 1);
+    hd_atomic_add(acc + gr * (P + 1) + pc, 1);
   }
   if (in_sh) {
-    PN_SYNC();
-    for (int c = PN_TID; c < ncell; c += PN_NT)
-      if (sh[c]) pn_add32(cells + c, sh[c]);
+    HD_SYNC();
+    for (int c = HD_TID; c < ncell; c += HD_NT)
+      if (sh[c]) hd_atomic_add(cells + c, sh[c]);
   }
 }
 
@@ -284,7 +255,7 @@ struct MatchShared {
   int crowd_of[kMaxCat];             // category -> crowd GT segment (last in JSON order), or -1
 };
 
-PN_FN void pq_match(const PqParams& p, int b, MatchShared& sh) {
+HD_FN void pq_match(const PqParams& p, int b, MatchShared& sh) {
   const int64_t* g = p.img + int64_t(b) * kPqFields;
   const int G = int(g[kPqG]), P = int(g[kPqP]), void_row = int(g[kPqVoidRow]);
   const int64_t go = g[kPqGtOff], po = g[kPqPredOff], row = g[kPqStatRow];
@@ -300,19 +271,19 @@ PN_FN void pq_match(const PqParams& p, int b, MatchShared& sh) {
   int32_t* st = p.stat_i + row * p.Kc * 3;
   double* siou = p.stat_iou + row * p.Kc;
   const int stride = P + 1;
-  for (int k = PN_TID; k < p.Kc; k += PN_NT) {
+  for (int k = HD_TID; k < p.Kc; k += HD_NT) {
     st[3 * k] = st[3 * k + 1] = st[3 * k + 2] = 0;
     siou[k] = 0.0;
     sh.crowd_of[k] = -1;
   }
-  for (int j = PN_TID; j < P; j += PN_NT) {
+  for (int j = HD_TID; j < P; j += HD_NT) {
     int64_t a = 0;
     for (int r = 0; r < G + 2; ++r) a += cells[r * stride + j];
     parea[j] = a;
     sh.pmatched[j] = 0;
   }
-  PN_SYNC();
-  if (PN_TID == 0) {                                     // the image's errors, as panopticapi meets them
+  HD_SYNC();
+  if (HD_TID == 0) {                                     // the image's errors, as panopticapi meets them
     long long cat_err = LLONG_MAX, missing = 0;
     for (int j = 0; j < P; ++j) {
       if (parea[j] == 0) ++missing;
@@ -321,7 +292,7 @@ PN_FN void pq_match(const PqParams& p, int b, MatchShared& sh) {
     err[kErrCategory] = cat_err;
     err[kErrMissing] = missing;
   }
-  for (int r = PN_TID; r < G; r += PN_NT) {
+  for (int r = HD_TID; r < G; r += HD_NT) {
     sh.match[r] = -1;
     sh.iou[r] = 0.0;
     if (gcrowd[r]) continue;
@@ -329,19 +300,19 @@ PN_FN void pq_match(const PqParams& p, int b, MatchShared& sh) {
     for (int j = 0; j < P; ++j) {
       const int inter = cells[r * stride + j];
       if (inter == 0 || pcat[j] != gcat[r]) continue;
-      const double uni = pn_dsub(pn_dsub(pn_dadd(double(parea[j]), garea[r]), double(inter)),
+      const double uni = hd_dsub(hd_dsub(hd_dadd(double(parea[j]), garea[r]), double(inter)),
                                  double(cells[void_inter_row + j]));
-      const double iou = pn_ddiv(double(inter), uni);
+      const double iou = hd_ddiv(double(inter), uni);
       if (iou > 0.5) { sh.match[r] = j; sh.iou[r] = iou; }
     }
   }
-  PN_SYNC();
-  if (PN_TID == 0) {
+  HD_SYNC();
+  if (HD_TID == 0) {
     for (int r = 0; r < G; ++r) {                        // ascending GT id: the order of np.unique's pair keys
       const int c = gcat[r];
       if (sh.match[r] >= 0) {
         sh.pmatched[sh.match[r]] = 1;
-        if (c >= 0) { st[3 * c] += 1; siou[c] = pn_dadd(siou[c], sh.iou[r]); }
+        if (c >= 0) { st[3 * c] += 1; siou[c] = hd_dadd(siou[c], sh.iou[r]); }
       } else if (gcrowd[r]) {
         if (c >= 0 && (sh.crowd_of[c] < 0 || gjson[sh.crowd_of[c]] < gjson[r])) sh.crowd_of[c] = r;
       } else if (c >= 0) {
@@ -353,7 +324,7 @@ PN_FN void pq_match(const PqParams& p, int b, MatchShared& sh) {
       if (sh.pmatched[j] || c < 0 || parea[j] == 0) continue;
       int64_t inter = cells[int64_t(void_row) * stride + j];
       if (sh.crowd_of[c] >= 0) inter += cells[int64_t(sh.crowd_of[c]) * stride + j];
-      if (pn_ddiv(double(inter), double(parea[j])) > 0.5) continue;
+      if (hd_ddiv(double(inter), double(parea[j])) > 0.5) continue;
       st[3 * c + 1] += 1;
     }
   }
@@ -361,7 +332,7 @@ PN_FN void pq_match(const PqParams& p, int b, MatchShared& sh) {
 
 // category k: sums over the records rows[0 .. n) in that order; out [Kc][4] tp, fp, fn, iou.  err_out[0] is the first
 // i whose record has an error (or n)
-PN_FN void pq_reduce(const int32_t* stat_i, const double* stat_iou, const long long* err, const int64_t* rows,
+HD_FN void pq_reduce(const int32_t* stat_i, const double* stat_iou, const long long* err, const int64_t* rows,
                      int64_t n, int Kc, int k, double* out, int64_t* err_out) {
   if (k < Kc) {
     int64_t tp = 0, fp = 0, fn = 0;
@@ -371,7 +342,7 @@ PN_FN void pq_reduce(const int32_t* stat_i, const double* stat_iou, const long l
       tp += stat_i[(r * Kc + k) * 3];
       fp += stat_i[(r * Kc + k) * 3 + 1];
       fn += stat_i[(r * Kc + k) * 3 + 2];
-      iou = pn_dadd(iou, stat_iou[r * Kc + k]);
+      iou = hd_dadd(iou, stat_iou[r * Kc + k]);
     }
     out[4 * k] = double(tp);
     out[4 * k + 1] = double(fp);

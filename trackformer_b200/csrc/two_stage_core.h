@@ -18,23 +18,9 @@
 #include <math.h>
 #include <stddef.h>
 #include <stdint.h>
-#include <string.h>
 
 #include "../../include/tfb200_fused.h"
-
-#if defined(__CUDACC__)
-#define TS_FN __device__ inline
-#define TS_SYNC() __syncthreads()
-#define TS_TID (int(threadIdx.x))
-#define TS_NT (int(blockDim.x))
-#define ts_atomic_add(p, v) atomicAdd((p), (v))
-#else
-#define TS_FN static inline
-#define TS_SYNC() ((void)0)
-#define TS_TID 0
-#define TS_NT 1
-template <class T> static inline T ts_atomic_add(T* p, T v) { T o = *p; *p = o + v; return o; }
-#endif
+#include "host_device.h"
 
 namespace tfb200_two_stage {
 
@@ -54,25 +40,25 @@ struct ProposalParams {
 };
 
 // the unpadded width (row 0) and height (column 0) of every level of image b
-TS_FN void ts_valid_counts(const ProposalParams& p, int b, int* vw, int* vh) {
-  for (int l = TS_TID; l < p.L; l += TS_NT) { vw[l] = 0; vh[l] = 0; }
-  TS_SYNC();
+HD_FN void ts_valid_counts(const ProposalParams& p, int b, int* vw, int* vh) {
+  for (int l = HD_TID; l < p.L; l += HD_NT) { vw[l] = 0; vh[l] = 0; }
+  HD_SYNC();
   if (p.mask == nullptr) {
-    for (int l = TS_TID; l < p.L; l += TS_NT) { vw[l] = p.W[l]; vh[l] = p.H[l]; }
+    for (int l = HD_TID; l < p.L; l += HD_NT) { vw[l] = p.W[l]; vh[l] = p.H[l]; }
   } else {
     const uint8_t* m = p.mask + size_t(b) * p.S;
     for (int l = 0; l < p.L; ++l) {
-      for (int x = TS_TID; x < p.W[l]; x += TS_NT)
-        if (!m[p.start[l] + x]) ts_atomic_add(&vw[l], 1);
-      for (int y = TS_TID; y < p.H[l]; y += TS_NT)
-        if (!m[p.start[l] + y * p.W[l]]) ts_atomic_add(&vh[l], 1);
+      for (int x = HD_TID; x < p.W[l]; x += HD_NT)
+        if (!m[p.start[l] + x]) hd_atomic_add(&vw[l], 1);
+      for (int y = HD_TID; y < p.H[l]; y += HD_NT)
+        if (!m[p.start[l] + y * p.W[l]]) hd_atomic_add(&vh[l], 1);
     }
   }
-  TS_SYNC();
+  HD_SYNC();
 }
 
 // proposal logits and valid flag of token s of image b; returns the flag
-TS_FN bool ts_proposal(const ProposalParams& p, int b, int s, const int* vw, const int* vh) {
+HD_FN bool ts_proposal(const ProposalParams& p, int b, int s, const int* vw, const int* vh) {
   int l = 0;
   while (l + 1 < p.L && s >= p.start[l + 1]) ++l;
   const int r = s - p.start[l], y = r / p.W[l], x = r - y * p.W[l];
@@ -113,26 +99,21 @@ struct SelectShared {
 };
 
 // order-preserving key: a > b as floats <=> key(a) > key(b) as unsigned (-0 ranks below +0)
-TS_FN uint32_t ts_key(float f) {
-#if defined(__CUDACC__)
-  const uint32_t u = __float_as_uint(f);
-#else
-  uint32_t u;
-  memcpy(&u, &f, 4);
-#endif
+HD_FN uint32_t ts_key(float f) {
+  const uint32_t u = hd_float_bits(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
-TS_FN void ts_select(const SelectParams& p, int b, SelectShared& sh) {
+HD_FN void ts_select(const SelectParams& p, int b, SelectShared& sh) {
   const int S = p.S, k = p.k;
   uint32_t* keys = p.keys + size_t(b) * S;
-  if (TS_TID == 0) { sh.prefix = 0; sh.hi_mask = 0; sh.krem = k; sh.taken = 0; }
+  if (HD_TID == 0) { sh.prefix = 0; sh.hi_mask = 0; sh.krem = k; sh.taken = 0; }
   for (int pass = 0; pass < 4; ++pass) {
     const int shift = 24 - 8 * pass;
-    for (int i = TS_TID; i < 256; i += TS_NT) sh.hist[i] = 0;
-    TS_SYNC();
+    for (int i = HD_TID; i < 256; i += HD_NT) sh.hist[i] = 0;
+    HD_SYNC();
     const uint32_t prefix = sh.prefix, hi = sh.hi_mask;
-    for (int s = TS_TID; s < S; s += TS_NT) {
+    for (int s = HD_TID; s < S; s += HD_NT) {
       uint32_t key;
       if (pass == 0) {
         key = ts_key(p.logits[(size_t(b) * S + s) * p.C]);
@@ -140,10 +121,10 @@ TS_FN void ts_select(const SelectParams& p, int b, SelectShared& sh) {
       } else {
         key = keys[s];
       }
-      if ((key & hi) == prefix) ts_atomic_add(&sh.hist[(key >> shift) & 255u], 1u);
+      if ((key & hi) == prefix) hd_atomic_add(&sh.hist[(key >> shift) & 255u], 1u);
     }
-    TS_SYNC();
-    if (TS_TID == 0) {
+    HD_SYNC();
+    if (HD_TID == 0) {
       int above = 0, bin = 255;
       for (; bin > 0; --bin) {
         if (above + int(sh.hist[bin]) >= sh.krem) break;
@@ -153,39 +134,39 @@ TS_FN void ts_select(const SelectParams& p, int b, SelectShared& sh) {
       sh.prefix |= uint32_t(bin) << shift;
       sh.hi_mask |= 0xffu << shift;
     }
-    TS_SYNC();
+    HD_SYNC();
   }
   // threshold key t = sh.prefix; krem of the tokens with key t are taken, the lowest token indices first
   const uint32_t t = sh.prefix;
   const int krem = sh.krem;
-  if (TS_TID == 0) sh.ngt = k - krem;
-  TS_SYNC();
+  if (HD_TID == 0) sh.ngt = k - krem;
+  HD_SYNC();
   const int ngt = sh.ngt;
-  const int nt = TS_NT, seg = (S + nt - 1) / nt;
-  const int s0 = TS_TID * seg, s1 = s0 + seg < S ? s0 + seg : S;
+  const int nt = HD_NT, seg = (S + nt - 1) / nt;
+  const int s0 = HD_TID * seg, s1 = s0 + seg < S ? s0 + seg : S;
   int ties = 0;
-  for (int s = TS_TID; s < S; s += TS_NT) {
+  for (int s = HD_TID; s < S; s += HD_NT) {
     const uint32_t key = keys[s];
     if (key > t) {
-      const int at = ts_atomic_add(&sh.taken, 1);
+      const int at = hd_atomic_add(&sh.taken, 1);
       sh.wkey[at] = key;
       sh.widx[at] = s;
     }
   }
   for (int s = s0; s < s1; ++s) ties += keys[s] == t;
-  sh.cnt[TS_TID] = ties;
-  TS_SYNC();
-  if (TS_TID == 0) {
+  sh.cnt[HD_TID] = ties;
+  HD_SYNC();
+  if (HD_TID == 0) {
     int acc = 0;
     for (int i = 0; i < nt; ++i) { const int c = sh.cnt[i]; sh.cnt[i] = acc; acc += c; }
   }
-  TS_SYNC();
-  int run = sh.cnt[TS_TID];
+  HD_SYNC();
+  int run = sh.cnt[HD_TID];
   for (int s = s0; s < s1 && run < krem; ++s)
     if (keys[s] == t) { sh.wkey[ngt + run] = t; sh.widx[ngt + run] = s; ++run; }
-  TS_SYNC();
+  HD_SYNC();
   // rank sort of the k winners: logit descending, token ascending (a total order)
-  for (int i = TS_TID; i < k; i += TS_NT) {
+  for (int i = HD_TID; i < k; i += HD_NT) {
     const uint32_t ki = sh.wkey[i];
     const int ii = sh.widx[i];
     int rank = 0;
@@ -195,22 +176,22 @@ TS_FN void ts_select(const SelectParams& p, int b, SelectShared& sh) {
     }
     sh.order[rank] = ii;
   }
-  TS_SYNC();
+  HD_SYNC();
 }
 
-TS_FN float ts_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
+HD_FN float ts_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-TS_FN void ts_select_outputs(const SelectParams& p, int b, const SelectShared& sh) {
+HD_FN void ts_select_outputs(const SelectParams& p, int b, const SelectShared& sh) {
   const int k = p.k;
-  for (int r = TS_TID; r < k; r += TS_NT) p.index[size_t(b) * k + r] = sh.order[r];
-  for (int e = TS_TID; e < k * 4; e += TS_NT) {
+  for (int r = HD_TID; r < k; r += HD_NT) p.index[size_t(b) * k + r] = sh.order[r];
+  for (int e = HD_TID; e < k * 4; e += HD_NT) {
     const int r = e >> 2, c = e & 3;
     const float u = p.unact[(size_t(b) * p.S + sh.order[r]) * 4 + c];
     p.boxes[size_t(b) * k * 4 + e] = u;
     p.ref[size_t(b) * k * 4 + e] = ts_sigmoid(u);
   }
   const float scale = 6.28318530717958647692f;          // float(2 * math.pi)
-  for (int e = TS_TID; e < k * 4 * kEmbed; e += TS_NT) {
+  for (int e = HD_TID; e < k * 4 * kEmbed; e += HD_NT) {
     const int r = e / (4 * kEmbed), c = (e / kEmbed) & 3, j = e % kEmbed;
     const float u = p.unact[(size_t(b) * p.S + sh.order[r]) * 4 + c];
     const float pos = (ts_sigmoid(u) * scale) / p.dim_t[j];
